@@ -1,6 +1,7 @@
-"""bench.py — denoising-steps/sec of the Latte hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py — denoising-steps/sec of the Latte hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dtype fp16|bf16] [--model Latte-XL/2]
+                    [--dump-outputs DIR]
 
 A "step" is one denoising step of `sample/sample.py`: ONE `forward_with_cfg` call on the CFG pair of a
 16x(4x32x32) latent video (B_model = 2) — BASELINE.json configs[1], Latte-XL/2 class-conditional 16x256x256.
@@ -9,12 +10,15 @@ independent replica with its own video (sample_ddp.py partitioning): weak scalin
 `value` = N * K / max-over-ranks device time.
 
 JSON keys beyond the base contract:
-  roofline     dominant kernel = the tcgen05 GEMM family (4 launches per block): algorithmic GEMM FLOPs per step /
+  roofline     dominant kernel = the wgmma GEMM family (4 launches per block): algorithmic GEMM FLOPs per step /
                summed GEMM device time of a step, measured with CUDA events recorded on the launching stream by the
                library's profiling hook in a SECOND instrumented pass of K steps (the headline pass records nothing)
   cpu_baseline the oracle port (oracle/latte_oracle.py, torch CPU fp32) timed on this box's host cores, rank 0, N=1
   e2e          same metric through the public module call with HOST pinned buffers: H2D of x, forward, D2H of the result
   --impl reference: times the CPU oracle port only (the reference is pure Python and cannot travel; its restatement can).
+  --dump-outputs DIR: after the timed steps, writes what the last timed step returned (the forward_with_cfg output, float32)
+               as DIR/out.npy.  Inputs and weights are seeded, so two builds run with the same arguments can be compared
+               output for output.
 """
 from __future__ import annotations
 
@@ -41,11 +45,24 @@ def load_peaks():
         d = json.load(open(p))
         return dict(tensor_burst=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     hbm=d["hbm_gbs"], source="measured (MEASURED_PEAKS.json)")
-    return dict(tensor_burst=1590.0, tensor_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(tensor_burst=989.0, tensor_sustained=989.0, hbm=3350.0,
+                source="NVIDIA H100 SXM data sheet (dense BF16, 700 W card), not a measured rate")
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each tensor as out_dir/<name>.npy in float32 (64 MB at most in all)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, v in arrays.items():
+        a = v.detach().float().cpu().numpy()
+        total += a.nbytes
+        assert total <= 64 << 20, "dump exceeds 64 MB"
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -228,7 +245,7 @@ def run_t2v(args):
            "config": {"workload": "LatteT2V (Latte-1 config) 16x512x512, B_model=2, 120 text tokens",
                       "algorithmic_tflop_per_step": fl / 1e12, "step_tflops_achieved": fl / (ms * 1e-3) / 1e12},
            "gpu_launches": int(sum(pn) // K),
-           "roofline": {"bound": "tensor", "kernel": "gemm_kernel<BN,EPI> (tcgen05)", "achieved": achieved, "peak": peaks["tensor_sustained"],
+           "roofline": {"bound": "tensor", "kernel": "gemm_kernel<BN,EPI> (wgmma)", "achieved": achieved, "peak": peaks["tensor_sustained"],
                         "unit": "TFLOP/s", "frac": achieved / peaks["tensor_sustained"], "traffic": None,
                         "peak_source": peaks["source"] + ", sustained figure", "gemm_ms_per_step": pm[0] / K,
                         "attn_ms_per_step": pm[1] / K, "ln_ms_per_step": pm[2] / K, "other_ms_per_step": pm[3] / K}}
@@ -416,9 +433,13 @@ def main():
     ap.add_argument("--model", default="Latte-XL/2")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-video", action="store_true", help="skip the measured 250-step video + VAE decode (profiler runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output as DIR/out.npy (float32) for output-for-output comparisons")
     ap.add_argument("--workload", default="latte", choices=["latte", "t2v"],
                     help="latte = BASELINE configs[1] (the bench line); t2v = configs[3] denoiser step, a secondary measurement")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "latte" or args.impl != "b200"):
+        ap.error("--dump-outputs is supported for the default workload (--workload latte --impl b200) only")
     if args.workload == "t2v":
         return run_t2v(args)
     if args.impl == "reference":
@@ -450,6 +471,7 @@ def main():
     out_host = [torch.empty(2, cfg.num_frames, cfg.out_channels, cfg.input_size, cfg.input_size).pin_memory() for _ in range(2)]
     out_ready = [torch.cuda.Event(), torch.cuda.Event()]
     e2e_count = [0]
+    last_out = [None]
 
     def barrier():
         if world > 1:
@@ -457,7 +479,8 @@ def main():
         torch.cuda.synchronize()
 
     def step_resident():
-        return net.forward_with_cfg(xd, td, y=yd, cfg_scale=7.0)
+        last_out[0] = net.forward_with_cfg(xd, td, y=yd, cfg_scale=7.0)
+        return last_out[0]
 
     def step_e2e():
         """One step as a serving loop issues it: H2D of this step's latents from pinned memory, the public module call, D2H of
@@ -492,6 +515,8 @@ def main():
             step_e2e()
         clocks.mark_begin()
         ms_total = timed(step_resident, K)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"out": last_out[0]})
         ms_e2e = timed(step_e2e, K)
         clocks.mark_end()
         clk = clocks.stop() if rank == 0 else None
@@ -554,7 +579,7 @@ def main():
         "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": args.dtype, "data": "synthetic",
         "config": {"workload": WORKLOAD.format(model=args.model),
-                   "l2": "no explicit flush: 1.35 GB of 16-bit weights stream through the 126 MB L2 every step",
+                   "l2": "no explicit flush: 1.35 GB of 16-bit weights stream through the 50 MB L2 every step",
                    "parallelism": f"replicas x{world} (sample_ddp partitioning), no data-path collective",
                    "algorithmic_tflop_per_step": step_flops / 1e12,
                    "step_tflops_achieved": step_flops / (ms_total / K * 1e-3) / 1e12},
@@ -565,7 +590,7 @@ def main():
         "sustained": {"ms_per_step": ms_sustained, "value": world * 1000.0 / ms_sustained, "steps": 250,
                       "note": "same step, 250 back-to-back calls (sustained clocks under the power cap); `value` above is the K-step burst"},
         "gpu_launches": int(launches),
-        "roofline": {"bound": "tensor", "kernel": "gemm_kernel<BN,EPI> (tcgen05, 4 launches/block)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_kernel<BN,EPI> (wgmma, 4 launches/block)",
                      "achieved": achieved, "peak": peaks["tensor_sustained"], "unit": "TFLOP/s",
                      "frac": achieved / peaks["tensor_sustained"], "traffic": traffic, "traffic_source": traffic_src,
                      "peak_source": peaks["source"] + ", sustained figure (kernel timed inside a long step)",

@@ -1,4 +1,4 @@
-/* latte_b200 — C ABI of the B200-native Latte denoiser hot path (liblatte_b200.so).
+/* latte_b200 — C ABI of the H100-native (sm_90a) Latte denoiser hot path (liblatte_b200.so).
  *
  * Drop-in boundary (SURVEY.md §8b): the reference's hot path is `Latte.forward` /
  * `Latte.forward_with_cfg` (Vchitect/Latte models/latte.py:314-398), a PyTorch nn.Module.  A binding
@@ -10,7 +10,7 @@
  *     TMA descriptors (pure functions of pointer + shape) and per-device kernel attributes, so a call may be
  *     captured into a CUDA graph and replayed (tests/test_gpu_graph.py);
  *   - return value 0 = ok, negative B200_ERR_* otherwise; text via b200_last_error() (thread-local);
- *   - sm_100 only: any other device returns B200_ERR_ARCH. There is no CPU fallback.
+ *   - sm_90 (Hopper) only: any other device returns B200_ERR_ARCH. There is no CPU fallback.
  * All matrices are row-major.  "16-bit" means IEEE fp16 (dtype = B200_FP16) or bfloat16 (B200_BF16).
  */
 #ifndef LATTE_B200_H
@@ -84,7 +84,7 @@ typedef struct B200LatteWeights {
   const float* fc2_b;      /*                             [depth][D]                      */
   const float* final_w;    /* final_layer.linear.weight   [p*p*out_channels, D]           */
   const float* final_b;    /* final_layer.linear.bias     [p*p*out_channels]              */
-  const void* final_w16;   /* 16-bit copy of final_w: the head then runs LN+modulate -> tcgen05 GEMM (N = p*p*out_channels,
+  const void* final_w16;   /* 16-bit copy of final_w: the head then runs LN+modulate -> wgmma GEMM (N = p*p*out_channels,
                               fp32 result) -> unpatchify; NULL keeps the fp32 CUDA-core head                 */
 } B200LatteWeights;
 
@@ -319,7 +319,7 @@ B200_API int b200_latte_forward_conditioned(const B200LatteShape* shape, const B
                                             const float* mod, int batch, int use_cfg, float cfg_scale, float* out,
                                             void* workspace, size_t workspace_bytes, void* stream);
 
-/* out = epilogue(A @ W^T + bias) on tcgen05 tensor cores — replaces the nn.Linear calls of the block
+/* out = epilogue(A @ W^T + bias) on wgmma tensor cores — replaces the nn.Linear calls of the block
  * (latte.py:50 qkv, :75 proj, timm Mlp fc1/fc2 via :171).  A [M,K], W [N,K] 16-bit; bias [N] fp32 or NULL.
  *   B200_EPI_BIAS           out16[M,N] = acc + bias
  *   B200_EPI_BIAS_GELU      out16[M,N] = gelu_tanh(acc + bias)                     (latte.py:169)
@@ -341,9 +341,9 @@ B200_API int b200_linear(const void* A, const void* W, const float* bias, int M,
 B200_API int b200_attention(const void* qkv, void* out, int batch, int frames, int tokens, int heads, int head_dim,
                    int dtype, int temporal, void* stream);
 
-/* A/B switch for the <= 256-key attention kernels (process-wide): 0 = library default (or B200_ATTN_IMPL from the
- * environment), 2 = the two-tile pipeline of round 1, 3 = the role-warp kernel (two warpgroups per 256-key tile,
- * three 128-key tiles in flight, TMA-stored output).  Both are exact implementations of the same contract.      */
+/* Attention-kernel selector, kept for ABI compatibility.  The sm_90a build has ONE attention forward kernel: 0 (default),
+ * 2 and 3 (the kernel generations of earlier builds) are accepted and all select it; other values return
+ * B200_ERR_UNSUPPORTED.                                                                                              */
 B200_API int b200_set_attention_impl(int impl);
 
 /* out16[r, :] = LayerNorm(x[r, :]; no affine, eps 1e-6) * (1 + scale[b]) + shift[b], b = r / rows_per_batch

@@ -1,4 +1,4 @@
-"""latte_b200 — B200-native (sm_100a) implementation of the Latte denoising hot path behind the
+"""latte_b200 — H100-native (sm_90a) implementation of the Latte denoising hot path behind the
 reference's own module surface.  See DESIGN.md / INTEGRATION.md."""
 from .latte import Latte, Latte_models  # noqa: F401
 from .latte_t2v import LatteT2V  # noqa: F401

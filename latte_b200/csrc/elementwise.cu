@@ -559,7 +559,7 @@ int launch_cast16(const float* in, void* out16, long long n, int bf16, cudaStrea
   B200_REQUIRE(n % 4 == 0, B200_ERR_SHAPE, "cast16: element count %lld must be a multiple of 4", n);
   const long long n4 = n / 4;
   int blocks = static_cast<int>((n4 + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (bf16) cast16_kernel<true><<<blocks, 256, 0, stream>>>(in, reinterpret_cast<uint16_t*>(out16), n4);
   else cast16_kernel<false><<<blocks, 256, 0, stream>>>(in, reinterpret_cast<uint16_t*>(out16), n4);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -701,7 +701,7 @@ int launch_frames_to_uint8(const void* video, int dtype, int n, int c, int h, in
   B200_REQUIRE(dtype >= 0 && dtype <= 2 && (mode == 0 || mode == 1), B200_ERR_UNSUPPORTED, "frames_to_uint8: dtype %d / mode %d", dtype, mode);
   const long long total = static_cast<long long>(n) * c * h * w;
   int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (dtype == 0) frames_to_uint8_kernel<0><<<blocks, 256, 0, stream>>>(video, out, total, c, h * w, mode);
   else if (dtype == 1) frames_to_uint8_kernel<1><<<blocks, 256, 0, stream>>>(video, out, total, c, h * w, mode);
   else frames_to_uint8_kernel<2><<<blocks, 256, 0, stream>>>(video, out, total, c, h * w, mode);
@@ -717,7 +717,7 @@ int launch_unpatchify(const float* y, float* out, int batch, int frames, int gri
   const long long sf = channels_first ? plane : plane * out_ch;
   const long long sc = channels_first ? plane * frames : plane;
   int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   unpatchify_kernel<<<blocks, 256, 0, stream>>>(y, out, total, frames, grid, patch, out_ch, patch * patch * out_ch, sb, sf, sc);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;

@@ -1,4 +1,4 @@
-// tcgen05 GEMM with fused epilogues: out = epi(A[M,K] @ W[N,K]^T + bias)
+// wgmma GEMM with fused epilogues: out = epi(A[M,K] @ W[N,K]^T + bias)
 //
 // Replaces the nn.Linear calls inside a Latte TransformerBlock (reference models/latte.py:50 qkv, :75 proj,
 // timm Mlp fc1/fc2 reached from :171,:180) together with the elementwise work that follows them:
@@ -7,32 +7,22 @@
 //   EPI_GATE_RESIDUAL  proj / fc2 + adaLN gate + residual add, fp32 residual stream in place
 //                      (latte.py:179-180), optionally + temp_embed rows        (latte.py:357-358)
 //
-// What bounds this kernel on B200 is the operand bytes each SM must keep in flight (latency x consumption rate), so
-// CTAs run as PAIRS (cluster of 2, tcgen05 cta_group::2): one 256 x BN tile per pair, M = 256 MMAs issued by the leader
-// CTA, each CTA staging its own 128 A rows and only HALF of the W tile (the pair's MMA reads both halves).  Per SM that
-// is 64 B per MMA cycle at BN = 256 instead of 96, and the freed shared memory buys a 6-deep TMA pipeline.
-//   * both CTAs' TMA loads complete on the LEADER's "full" barrier (cta_group::2 loads, expect_tx = 2 stages); the peer's
-//     producer adds one plain remote arrive per stage (NOT .release.cluster: that fence cost 1.5k cycles per k-block);
-//   * the leader's tcgen05.commit is multicast to both CTAs' "empty" and "accumulator full" barriers;
-//   * both CTAs' epilogue warps release an accumulator on the leader's "accumulator empty" barrier (8 arrivals).
+// Hopper structure: CTAs run as PAIRS (cluster of 2).  A pair owns a 256 x BN pair-tile: each CTA multiplies its own 128 A
+// rows, and each fetches only HALF of the W tile and multicasts it into both CTAs' shared memory (TMA .multicast::cluster),
+// so every W byte crosses L2 -> SM once per pair.
+//   thread 0        also the TMA producer: A tile 128x64 and the W half (BN/2)x64 (128B-swizzled) per pipeline stage;
+//                   a stage is full when this CTA's A bytes and BOTH W halves have landed on its "full" barrier.  (A
+//                   separate producer warp would cap every thread at 168 registers; the 64 x 256 accumulator needs 128.)
+//   warpgroups 0-1  wgmma (64 x BN x 16, fp32 accumulators in registers), one 64-row half of the tile each, then the
+//                   epilogue straight from the accumulator registers; a stage is released with one arrival per warpgroup on
+//                   the "empty" barriers of BOTH CTAs (the peer's next multicast writes into it)
 //
-// Structure (one persistent CTA per SM, 224 threads, pair-tiles visited n-fastest so concurrent clusters share A panels in L2):
-//   warp 0      TMA producer: A tile 128x64 and W half-tile (BN/2)x64 (128B-swizzled) per pipeline stage
-//   warp 1      TMEM allocator; in the leader CTA also the single-thread tcgen05.mma issuer (M=256, N=BN, K=16)
-//   warps 2..5  epilogue warpgroup 0 (thread = accumulator row = TMEM lane)
-//   warps 6..9  epilogue warpgroup 1 (16-bit output modes: the two groups take alternate 64-column chunks; with one
-//               warp per scheduler the epilogue is instruction-latency bound, two warps per scheduler hide it)
-//   warp 10     spare
-// Two accumulator buffers in TMEM (2*BN columns) let the epilogue of tile i overlap the mainloop of tile i+1.
-//
-// Epilogue data movement is shaped so that every global access is a whole 128-byte line:
-//   16-bit outputs:  registers -> smem staging tile (rows of 128 B, 16-byte chunks XOR-swizzled by row%8, conflict-free)
-//                    -> re-read with 8 threads per row -> coalesced 16-byte stores.
-//   residual:        x is never loaded: the delta gate*(acc+bias) goes to a swizzled smem tile and a TMA reduce-add
-//                    (cp.reduce.async.bulk.tensor ... .add, fp32) folds it into the residual stream in L2.
+// Residual epilogue: every element of x is owned by one thread and updated in place (x += gate * (acc + bias) (+ row_add)),
+// once per GEMM -- or, for the stream-K tiles of the last waves, once per K segment in k order (TileSched below).
 #include <cstdio>
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 #include <cstdlib>
 
@@ -42,26 +32,22 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 x 16-bit = one 128-byte swizzle row
-constexpr int kThreads = 352;   // warps: 0 TMA, 1 MMA/forwarder, 2-5 epilogue WG0, 6-9 epilogue WG1, 10 residual loader
-constexpr int kSlotBytes = 128 * 128;  // one epilogue tile: 128 rows x 128 bytes
+constexpr int kThreads = 256;   // warpgroups 0-1 MMA + epilogue; thread 0 also issues the TMA loads
 
 template <int BN, int EPI>
 struct Cfg {
   static constexpr bool RESID = EPI == B200_EPI_GATE_RESIDUAL;
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;                // this CTA's half of the W tile
+  static constexpr int B_BYTES = BN * BK * 2;                       // the whole W tile (both CTAs' halves)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // residual: 2 staging tiles per epilogue warpgroup (TMA reduce-add sources); else: 1 per warpgroup
-  static constexpr int XSLOTS = RESID ? 4 : 2;
-  static constexpr int STAGES = RESID ? (BN >= 256 ? 5 : (BN >= 192 ? 5 : 6)) : (BN >= 256 ? 6 : (BN >= 192 ? 6 : 8));
-  static constexpr int TMEM_COLS = (2 * BN <= 256) ? 256 : 512;
-  static constexpr int BAR_BYTES = 512;
-  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;            // 1 KiB aligned (TMA 128B-swizzle boxes live here)
-  static constexpr int BAR_OFF = EPI_OFF + XSLOTS * kSlotBytes;
-  static constexpr int SMEM_BYTES = BAR_OFF + BAR_BYTES + 1024;   // +1024: manual 1 KiB alignment of the base
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int STAGES_FIT = (232448 - BAR_BYTES - 1024) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // BN 256: 4, 192: 5, 128: 7
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFF + BAR_BYTES + 1024;    // +1024: manual 1 KiB alignment of the base
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1 KiB alignment");
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
-  static_assert(3 * STAGES + 4 + 2 * XSLOTS + 1 <= BAR_BYTES / 8, "barrier area too small");
+  static_assert(2 * STAGES <= BAR_BYTES / 8, "barrier area too small");
 };
 
 struct GemmDev {
@@ -79,16 +65,15 @@ struct GemmDev {
   // implicit-GEMM convolution: see GemmArgs
   int conv_taps, conv_cblk, conv_h, conv_w, conv_bw, conv_bh;
   int conv_dx[9], conv_dy[9], conv_dz[9];
-  int w_const;  // W is a weight (not produced by a kernel of the step): its first tiles may be fetched before griddepcontrol.wait
   int mn_major; // bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (the contraction dimension is the ROW index): such an
-                // operand is fetched as 64-wide MN chunks x 64 k-rows and multiplied through an MN-major UMMA descriptor.
+                // operand is fetched as 64-wide MN blocks x 64 k-rows and multiplied through an MN-major wgmma descriptor.
                 // wgrad sets both (dW = dY^T X), dgrad only bit 1 (dX = dY W with W in its [out, in] layout).
+  float* resid; // EPI_GATE_RESIDUAL: [M, N] fp32 residual stream, updated in place
   int streamk;  // residual epilogue only: split the last partial wave of tiles along K across all pairs (see TileSched)
   // stream-K ordering flags (caller's workspace), one per (streamed tile, CTA rank, epilogue warpgroup): "k-blocks of the
   // tile already added into x".  All zero between launches: the segment that completes a tile resets its flag, so the
   // protocol holds no host-side state and a captured CUDA graph replays it unchanged.
   unsigned long long* sk_flags;
-  int dbg;  // timing experiments only (results are wrong when set): bit0 = no operand TMA, bit1 = no MMA issue, bit2 = no 16-bit epilogue
 };
 
 __device__ __forceinline__ void flag_release(unsigned long long* f, unsigned long long v) {
@@ -100,14 +85,10 @@ __device__ __forceinline__ void flag_wait(const unsigned long long* f, unsigned 
     unsigned long long v;
     asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(f) : "memory");
     if (v == want) return;
-    if (clock64() - t0 > 4000000000LL) {   // ~2 s: a protocol bug must not hang the GPU
-      printf("gemm: stream-K flag wait timed out (block %d)\n", blockIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s: a protocol bug must not hang the GPU (no printf: see mbar_wait)
     __nanosleep(64);
   }
 }
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
 // Work schedule of one CTA pair.  Data-parallel part: pair k owns tiles k, k + P, ... for the `full_waves` complete waves.
 // Stream-K part (residual epilogue only, where partial sums can be reduce-added into x): the tiles of the last, partial
@@ -166,8 +147,8 @@ __device__ __forceinline__ float gelu_tanh_grad(float x) {
 
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5 x (1 + tanh(u)),  u = sqrt(2/pi) (x + 0.044715 x^3).  ONE MUFU op per element (tanh.approx, rel. error 2^-11,
-  // the same size as the 16-bit rounding of the result): with ex2 + rcp (two MUFU ops) the fc1 epilogue was bound by the
-  // 16/clk/SM MUFU pipe (r01 experiment: 4.9k cycles per 128x256 tile).
+  // the same size as the 16-bit rounding of the result) instead of ex2 + rcp: the 16/clk/SM MUFU pipe is the fc1
+  // epilogue's narrowest resource.
   const float u = 0.7978845608028654f * fmaf(0.044715f * x * x, x, x);
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
@@ -177,21 +158,13 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 
 template <int BN, int EPI, bool BF16>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmX, const GemmDev p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
   using C = Cfg<BN, EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_smem = smem + C::EPI_OFF;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
   uint64_t* full = bars;
   uint64_t* empty = bars + C::STAGES;
-  uint64_t* pfull = bars + 2 * C::STAGES;   // leader only: "the peer's stage has landed"
-  uint64_t* tfull = bars + 3 * C::STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* xfull = tempty + 2;
-  uint64_t* xempty = xfull + C::XSLOTS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(xempty + C::XSLOTS);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -199,32 +172,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if constexpr (C::RESID) tma_prefetch_desc(&tmX);
     for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full[i], 2);    // (leader's copy is the live one) leader's expect_tx arrival + the peer's arrival
-      mbar_init(&pfull[i], 1);   // unused
-      mbar_init(&empty[i], 1);   // leader's tcgen05.commit, multicast to both CTAs
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);   // leader's tcgen05.commit, multicast to both CTAs
-      mbar_init(&tempty[i], 16); // (leader's copy) one arrival per epilogue warp of BOTH CTAs
-    }
-    for (int i = 0; i < C::XSLOTS; ++i) {
-      mbar_init(&xfull[i], 1);
-      mbar_init(&xempty[i], 1);
+      mbar_init(&full[i], 1);    // this CTA's expect_tx arrival; the bytes of both W halves and of A complete it
+      mbar_init(&empty[i], 4);   // one arrival per MMA warpgroup of BOTH CTAs (each W half lands in both)
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();      // CTA-scope order for the allocator's write of tmem_slot (what compute-sanitizer's racecheck models;
-                        // the cluster barrier below already implies it)
   cluster_sync_all();   // barriers of both CTAs are initialised before any multicast / remote arrival can target them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();   // the next kernel may begin its prologue as SMs drain
-  // griddepcontrol.wait (the predecessor's outputs become visible) is executed by each role that touches global memory --
-  // the producer only AFTER it has put the first W tiles in flight when W is a constant weight (see below)
 
   // pair-tile schedule: cluster k owns pair-tiles k, k + #clusters, ...; a pair-tile is two M-adjacent 128-row tiles of
   // one N column; this CTA takes row-tile 2 * pair_m + rank (it may lie past M: zero-filled loads, clipped stores)
@@ -235,394 +190,249 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int num_pairs = gridDim.x >> 1;
   const int num_kb = p.K / BK;
   const bool streamk = C::RESID && p.streamk != 0;
-  const bool leader = rank == 0;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (operands)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      // W tiles of the first k-blocks are fetched BEFORE the grid dependency resolves when W is a weight (never written by
-      // a kernel of the step): they come from DRAM (1.35 GB of weights stream through L2 every step), the A tiles from the
-      // L2 the predecessor just filled, so this takes the longer of the two latencies off the start of every GEMM.
-      int prefetched = 0;
-      if (p.w_const && !(p.dbg & 1)) {
-        TileSched s0(my_pair, num_pairs, num_tiles, num_kb, streamk);
-        int t0, k0, k1;
-        if (s0.next(t0, k0, k1)) {
-          const int n_blk = t0 % p.num_n;
-          const int n_live = ((p.N - n_blk * BN) < BN && !(p.dbg & 64)) ? (p.N - n_blk * BN) : BN;
-          const int w_row0 = n_blk * BN + static_cast<int>(rank) * (n_live / 2);
-          prefetched = (k1 - k0) < C::STAGES ? (k1 - k0) : C::STAGES;
-          for (int i = 0; i < prefetched; ++i) {
-            const uint32_t full_leader = mapa_u32(&full[i], 0);
-            if (leader) mbar_arrive_expect_tx(&full[i], 2 * C::STAGE_BYTES);
-            else mbar_arrive_cluster(full_leader);
-            tma_load_2d_pair(smem + i * C::STAGE_BYTES + C::A_BYTES, &tmB, full_leader, (k0 + i) * BK, w_row0);
+  // ------------------------------------------------------------------ TMA producer (thread 0, between its own MMAs)
+  // Load q of this CTA's k-block sequence goes to slot q % STAGES; it is issued once the slot's previous contents (load
+  // q - STAGES) have been released by both warpgroups of both CTAs.  Loads run up to STAGES - 1 k-blocks ahead of the MMAs,
+  // across tile boundaries, so the next tile's operands stream in while the epilogue runs.
+  TileSched lsched(my_pair, num_pairs, num_tiles, num_kb, streamk);
+  int l_tile = 0, l_kb = 0, l_kb1 = 0;
+  long long issued = 0;
+  bool l_more = true;
+  auto issue_one = [&]() {
+    if (l_kb == l_kb1) {
+      if (!(l_more = lsched.next(l_tile, l_kb, l_kb1))) return;
+    }
+    const int stage = static_cast<int>(issued % C::STAGES);
+    const uint32_t phase = static_cast<uint32_t>(issued / C::STAGES) & 1u;
+    const int m_blk = 2 * (l_tile / p.num_n) + static_cast<int>(rank), n_blk = l_tile % p.num_n;
+    const int w_row0 = n_blk * BN + static_cast<int>(rank) * (BN / 2);   // this CTA fetches half of the W tile for both
+    const int kb = l_kb++;
+    ++issued;
+    mbar_wait(&empty[stage], phase ^ 1);        // both CTAs' warpgroups are done with the slot
+    mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
+    uint8_t* sa = smem + stage * C::STAGE_BYTES;
+    if (p.conv_taps > 0) {
+      // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
+      // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
+      const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
+      const int pix0 = m_blk * BM;
+      const int hw = p.conv_h * p.conv_w;
+      const int img = pix0 / hw, rem = pix0 % hw;
+      tma_load_4d(sa, &tmA, &full[stage], cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap],
+                  img + p.conv_dz[tap]);
+    } else if (p.mn_major & 1) {
+      // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
+      // MN-major SW128 block; blocks past the live rows are zero-filled by TMA and still count their bytes
+#pragma unroll
+      for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, &full[stage], m_blk * BM + j * 64, kb * BK);
+    } else {
+      tma_load_2d(sa, &tmA, &full[stage], kb * BK, m_blk * BM);
+    }
+    if (p.mn_major & 2) {
+      constexpr int per_cta = BN / 128;          // 64-column blocks of W this CTA fetches
+#pragma unroll
+      for (int j = 0; j < per_cta; ++j)
+        tma_load_2d_mcast(sa + C::A_BYTES + (rank * per_cta + j) * 8192, &tmB, &full[stage], w_row0 + j * 64, kb * BK, 0x3);
+    } else {
+      tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK, w_row0, 0x3);
+    }
+  };
+
+  pdl_wait();                                 // operands, bias / gate / shortcut / residual stream: visible from here
+  const bool producer = threadIdx.x == 0;
+  if (producer)
+    for (int i = 0; i < C::STAGES - 1 && l_more; ++i) issue_one();
+  {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroups 0, 1 (64 rows each)
+    const int wg = warp >> 2;
+    const int te = threadIdx.x & 127;
+    const int w4 = te >> 5, g = lane >> 2, cq = lane & 3;
+    const uint32_t empty_peer = mapa_u32(&empty[0], rank ^ 1u);
+    int stage = 0;
+    uint32_t phase = 0;
+    long long consumed = 0;
+    float acc[BN / 2];
+    TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
+    int tile, kb0, kb1;
+    while (sched.next(tile, kb0, kb1)) {
+      const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN;
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES), sb = sa + C::A_BYTES;
+        wgmma_fence();
+        // K-major: 8-row groups 1024 B apart, a k-step of 16 elements = 32 B inside the swizzle row.  MN-major: 64-wide
+        // blocks 8192 B apart (leading offset), 8-k-row groups 1024 B apart, a k-step of 16 k-rows = 2048 B.
+        switch (p.mn_major) {
+          case 0: {
+            const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+              WgmmaSS<BN, 0, 0, BF16>::mma(acc, gmma_desc_advance(da, k * 32), gmma_desc_advance(db, k * 32), (kb != kb0 || k) ? 1u : 0u);
+            break;
+          }
+          case 2: {
+            const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 8192, 1024, GMMA_LAYOUT_SW128);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+              WgmmaSS<BN, 0, 1, BF16>::mma(acc, gmma_desc_advance(da, k * 32), gmma_desc_advance(db, k * 2048), (kb != kb0 || k) ? 1u : 0u);
+            break;
+          }
+          case 1: {
+            const uint64_t da = gmma_desc(sa + wg * 8192, 8192, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+              WgmmaSS<BN, 1, 0, BF16>::mma(acc, gmma_desc_advance(da, k * 2048), gmma_desc_advance(db, k * 32), (kb != kb0 || k) ? 1u : 0u);
+            break;
+          }
+          default: {
+            const uint64_t da = gmma_desc(sa + wg * 8192, 8192, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 8192, 1024, GMMA_LAYOUT_SW128);
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+              WgmmaSS<BN, 1, 1, BF16>::mma(acc, gmma_desc_advance(da, k * 2048), gmma_desc_advance(db, k * 2048), (kb != kb0 || k) ? 1u : 0u);
+            break;
           }
         }
-      }
-      pdl_wait();
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
-        const int m_blk = 2 * (tile / p.num_n) + static_cast<int>(rank), n_blk = tile % p.num_n;
-        // narrow edge tile (N not a multiple of BN): the pair's MMA shrinks to the live columns (see the MMA warp), so the two
-        // halves of the W tile are the two halves of the LIVE columns
-        const int n_live = ((p.N - n_blk * BN) < BN && !(p.dbg & 64)) ? (p.N - n_blk * BN) : BN;
-        const int w_row0 = n_blk * BN + static_cast<int>(rank) * (n_live / 2);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          const bool w_in_flight = prefetched > 0;     // this stage's expect_tx / arrival and W load were issued above
-          if (w_in_flight) --prefetched;
-          else mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * C::STAGE_BYTES;
-          const uint32_t full_leader = mapa_u32(&full[stage], 0);
-          if (p.dbg & 1) {
-            if (leader) mbar_arrive(&full[stage]); else mbar_arrive_cluster(full_leader);
-          } else {
-            // both CTAs' bytes complete on the LEADER's barrier (cta_group::2 loads may signal the pair leader)
-            if (!w_in_flight) {
-              if (leader) mbar_arrive_expect_tx(&full[stage], 2 * C::STAGE_BYTES);
-              else mbar_arrive_cluster(full_leader);
-            }
-            if (p.conv_taps > 0) {
-              // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
-              // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
-              const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
-              const int pix0 = m_blk * BM;
-              const int hw = p.conv_h * p.conv_w;
-              const int img = pix0 / hw, rem = pix0 % hw;
-              tma_load_4d_pair(sa, &tmA, full_leader, cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap], img + p.conv_dz[tap]);
-            } else if (p.mn_major & 1) {
-              // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
-              // MN-major SW128 chunk; chunks past the live columns / rows are zero-filled by TMA and still count their bytes
-#pragma unroll
-              for (int j = 0; j < BM / 64; ++j) tma_load_2d_pair(sa + j * 8192, &tmA, full_leader, m_blk * BM + j * 64, kb * BK);
-            } else {
-              tma_load_2d_pair(sa, &tmA, full_leader, kb * BK, m_blk * BM);
-            }
-            if (p.mn_major & 2) {
-#pragma unroll
-              for (int j = 0; j < BN / 128; ++j)
-                tma_load_2d_pair(sa + C::A_BYTES + j * 8192, &tmB, full_leader, w_row0 + j * 64, kb * BK);
-            } else if (!w_in_flight) {
-              tma_load_2d_pair(sa + C::A_BYTES, &tmB, full_leader, kb * BK, w_row0);
-            }
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        wgmma_commit();
+        wgmma_wait<1>();                      // the previous k-block's MMAs have read their slot: release it in both CTAs
+        if (prev >= 0 && te == 0) {
+          mbar_arrive(&empty[prev]);
+          mbar_arrive_cluster(empty_peer + prev * 8);
         }
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        ++consumed;
+        if (producer)
+          while (l_more && issued < consumed + C::STAGES - 1) issue_one();
       }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread of the leader CTA)
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc_full = umma_idesc_f16(BF16, 2 * BM, BN, false, false);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        // edge tile: only the live columns (a multiple of 32) are multiplied -- no tensor work / energy on zero padding
-        const int n0 = (tile % p.num_n) * BN;
-        const int n_live = ((p.N - n0) < BN && !(p.dbg & 64)) ? (p.N - n0) : BN;   // dbg bit 6: A/B switch (full-width edge tiles)
-        const bool a_mn = (p.mn_major & 1) != 0, b_mn = (p.mn_major & 2) != 0;
-        const uint32_t idesc = (n_live == BN && !p.mn_major) ? idesc_full
-                                                             : umma_idesc_f16(BF16, 2 * BM, static_cast<uint32_t>(n_live), a_mn, b_mn);
-        // K-major: 8-row groups 1024 B apart, a k-step of 16 elements = 32 B inside the swizzle row.  MN-major: 64-wide MN
-        // chunks 8192 B apart (leading offset), 8-k-row groups 1024 B apart, a k-step of 16 k-rows = 2048 B.
-        const uint32_t lbo_a = a_mn ? 8192u : 0u, kstep_a = a_mn ? 2048u : 32u;
-        const uint32_t lbo_b = b_mn ? 8192u : 0u, kstep_b = b_mn ? 2048u : 32u;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);            // both CTAs' operands landed
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint64_t da = umma_smem_desc(sa, lbo_a, 1024, UMMA_LAYOUT_SW128);
-          const uint64_t db = umma_smem_desc(sa + C::A_BYTES, lbo_b, 1024, UMMA_LAYOUT_SW128);
-          if (!(p.dbg & 2))
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_f16_ss_pair(d_tmem, umma_desc_advance(da, k * kstep_a), umma_desc_advance(db, k * kstep_b), idesc,
-                             (kb != kb0 || k != 0) ? 1u : 0u);
-          umma_commit_pair(&empty[stage], 0x3);  // slot reusable in BOTH CTAs once these MMAs have read it
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_pair(&tfull[acc], 0x3);      // accumulator complete -> both CTAs' epilogues
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (te == 0) {
+        mbar_arrive(&empty[prev]);
+        mbar_arrive_cluster(empty_peer + prev * 8);
       }
-    }
-  } else if (warp == 10) {
-    // spare warp (kept so the warp-role layout is the same for every epilogue mode)
-  } else {
-    // ------------------------------------------------------------------ epilogue warps 2..9
-    pdl_wait();                               // bias / gate / shortcut / residual stream: visible from here
-    const int q = warp & 3;                   // TMEM lane quarter this warp may read
-    const int row_a = q * 32 + lane;          // accumulator row of this thread
-    const int wg = warp >= 6 ? 1 : 0;         // epilogue warpgroup
-    const int te = threadIdx.x - 64 - wg * 128;  // 0..127 within the warpgroup
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const uint32_t tempty_leader[2] = {mapa_u32(&tempty[0], 0), mapa_u32(&tempty[1], 0)};
 
-    if constexpr (C::RESID) {
-      // x += gate * (acc + bias) (+ row_add) WITHOUT loading x: the delta tile goes registers -> smem (128-byte rows,
-      // 16-byte chunks XOR-swizzled to match the tensor map) -> TMA reduce-add into the fp32 residual stream.  Each
-      // element receives one add per GEMM -- or, for stream-K tiles, one per segment in a fixed (k) order -- so results
-      // are deterministic.  The two warpgroups take alternate 32-column chunks (owner = running chunk counter & 1, or
-      // the chunk's own parity for stream-K so that a column always belongs to the same warpgroup) and double-buffer
-      // their own two staging tiles.
-      uint32_t cc = 0, mine = 0;
-      const int bar_a = 1 + 2 * wg, bar_b = 2 + 2 * wg;
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
+      // accumulator fragment: thread (w4, g, cq) holds rows r0 = 16*w4 + g and r0 + 8 of its 64, columns 8j + 2cq + {0,1}
+      const int r0 = m0 + wg * 64 + w4 * 16 + g;
+      if constexpr (C::RESID) {
+        // x += gate * (acc + bias) (+ row_add): every element belongs to one thread and receives one add per GEMM -- or,
+        // for stream-K tiles, one per segment in k order (the flag of the tile's rows of this warpgroup) -- so results
+        // are deterministic
         const bool first_seg = kb0 == 0;       // bias and row_add are added once per output element
-        const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN;
-        const uint32_t t_row = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16);
-        const int row = m0 + row_a;
-        const int row_c = row < p.M ? row : p.M - 1;  // rows past M produce deltas that the TMA store clips
-        const float* gate_row = p.gate + static_cast<long long>(row_c / p.rows_per_batch) * p.gate_bs;
-        const float* add_row = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((row_c / p.row_add_div) % p.row_add_period) * p.N : nullptr;
-        constexpr int NCH = BN / 32;
-        const int live = (p.N - n0) / 32 < NCH ? (p.N - n0) / 32 : NCH;   // chunks inside N (N % 32 == 0)
-        const uint32_t cbase = streamk ? 0u : cc;
-        int last_mine = -1;
-        for (int c = 0; c < live; ++c)
-          if (((cbase + c) & 1) == static_cast<uint32_t>(wg)) last_mine = c;
-        // stream-K ordering: this warpgroup's adds for the tile follow those of the segment that ends at kb0
         const bool partial = kb0 > 0 || kb1 < num_kb;
         unsigned long long* flag = nullptr;
         if (partial) flag = p.sk_flags + (static_cast<size_t>(tile - sched.full_waves * num_pairs) * 2 + rank) * 2 + wg;
-        bool must_wait = kb0 > 0;
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
-        if (last_mine < 0) {                   // a one-chunk edge tile owned by the other warpgroup
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(tempty_leader[acc]);
-        }
-#pragma unroll 1
-        for (int c = 0; c < live; ++c) {
-          if (((cbase + c) & 1) != static_cast<uint32_t>(wg)) continue;
-          const int col0 = n0 + c * 32;
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(t_row + c * 32, v);
-          tmem_ld_wait();
-          if (c == last_mine) {                // all of this warp's TMEM reads of the tile are done
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(tempty_leader[acc]);
-          }
-          if (p.dbg & 8) continue;     // timing experiment: accumulator read only
-          uint8_t* slot = epi_smem + (wg * 2 + (mine & 1)) * kSlotBytes;
-          ++mine;
-          uint8_t* drow = slot + row_a * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias && first_seg) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + j);
-            const float4 gt = __ldg(reinterpret_cast<const float4*>(gate_row + col0) + j);
-            float4 dv;
-            dv.x = gt.x * (__uint_as_float(v[4 * j + 0]) + b4.x);
-            dv.y = gt.y * (__uint_as_float(v[4 * j + 1]) + b4.y);
-            dv.z = gt.z * (__uint_as_float(v[4 * j + 2]) + b4.z);
-            dv.w = gt.w * (__uint_as_float(v[4 * j + 3]) + b4.w);
-            if (add_row) {
-              const float4 ra = __ldg(reinterpret_cast<const float4*>(add_row + col0) + j);
-              dv.x += ra.x; dv.y += ra.y; dv.z += ra.z; dv.w += ra.w;
-            }
-            *reinterpret_cast<float4*>(drow + ((j ^ (row_a & 7)) << 4)) = dv;
-          }
-          fence_proxy_async_smem();                     // generic-proxy smem writes -> visible to the TMA engine
-          asm volatile("bar.sync %0, 128;" ::"r"(bar_a) : "memory");
+        if (kb0 > 0) {
           if (te == 0) {
-            if (must_wait) {
-              flag_wait(flag, static_cast<unsigned long long>(kb0));
-              // nobody else waits on this flag; the segment that completes the tile leaves it zero for the next launch
-              if (kb1 == num_kb) flag_release(flag, 0ull);
-              fence_proxy_async_all();
-            }
-            tma_reduce_add_2d(&tmX, slot, col0, m0);
-            tma_store_commit();
-            tma_store_wait_read<1>();                   // the reduce issued one chunk ago (other tile) has read its smem
+            flag_wait(flag, static_cast<unsigned long long>(kb0));
+            // nobody else waits on this flag; the segment that completes the tile leaves it zero for the next launch
+            if (kb1 == num_kb) flag_release(flag, 0ull);
           }
-          must_wait = false;
-          asm volatile("bar.sync %0, 128;" ::"r"(bar_b) : "memory");   // ... so the other staging tile may be rewritten
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
         }
-        if (partial && kb1 < num_kb && last_mine >= 0 && te == 0 && !(p.dbg & 8)) {
-          tma_store_wait_all<0>();                      // this segment's adds have been performed ...
-          __threadfence();
-          flag_release(flag, static_cast<unsigned long long>(kb1));   // ... the next segment may add
-        }
-        cc += live;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (te == 0) tma_store_wait_all<0>();             // all residual updates have landed before the CTA retires
-    } else {
-      const int row_b0 = te >> 3;             // phase-B row within a group of 16
-      const int ch_b = te & 7;                // phase-B 16-byte chunk within the 128-byte row segment
-      uint8_t* buf = epi_smem + wg * kSlotBytes;   // one staging tile per warpgroup
-      const int bar_a = 1 + 2 * wg, bar_b = 2 + 2 * wg;
-      uint32_t cc = 0;                        // running chunk counter: chunk cc belongs to warpgroup (cc & 1)
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, false);
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
-        const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN;
-        const uint32_t t_row = tmem_base + acc * BN + (static_cast<uint32_t>(q * 32) << 16);
-        constexpr int NCH = BN / 64;           // 64 16-bit columns = 128 bytes per row per chunk
-        // this warpgroup's last chunk of the tile (after it the accumulator is no longer read by us)
-        int last_mine = -1;
 #pragma unroll
-        for (int c = 0; c < NCH; ++c)
-          if (((cc + c) & 1) == static_cast<uint32_t>(wg)) last_mine = c;
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
-        if (last_mine < 0) {                   // cannot happen for NCH >= 2, kept for safety
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(tempty_leader[acc]);
-        }
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) {
-          if (((cc + c) & 1) != static_cast<uint32_t>(wg)) continue;
-          uint32_t v0[32], v1[32];
-          tmem_ld_32x32b_x32(t_row + c * 64, v0);
-          tmem_ld_32x32b_x32(t_row + c * 64 + 32, v1);
-          tmem_ld_wait();
-          if (c == last_mine) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(tempty_leader[acc]);
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= p.M) continue;
+          const float* gate_row = p.gate + static_cast<long long>(row / p.rows_per_batch) * p.gate_bs;
+          const float* add_row = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((row / p.row_add_div) % p.row_add_period) * p.N : nullptr;
+          float* xrow = p.resid + static_cast<size_t>(row) * p.N;
+          const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j >= live) break;
+            const int col = n0 + 8 * j + 2 * cq;
+            float2 b2 = make_float2(0.f, 0.f);
+            if (p.bias && first_seg) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+            const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
+            float2 dv = make_float2(gt.x * (acc[4 * j + 2 * h] + b2.x), gt.y * (acc[4 * j + 2 * h + 1] + b2.y));
+            if (add_row) {
+              const float2 ra = __ldg(reinterpret_cast<const float2*>(add_row + col));
+              dv.x += ra.x; dv.y += ra.y;
+            }
+            float2 x = *reinterpret_cast<const float2*>(xrow + col);
+            x.x += dv.x; x.y += dv.y;
+            *reinterpret_cast<float2*>(xrow + col) = x;
           }
-          if (p.dbg & 4) continue;   // timing experiment: accumulator read only
-          const int col0 = n0 + c * 64;
-          uint8_t* srow = buf + row_a * 128;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            float f[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(hh ? v1[j] : v0[j]);
-            const int cb = col0 + hh * 32;
-            if (p.bias && cb < p.N) {
-              const float4* b4 = reinterpret_cast<const float4*>(p.bias + cb);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 b = __ldg(b4 + j);
-                f[4 * j + 0] += b.x; f[4 * j + 1] += b.y; f[4 * j + 2] += b.z; f[4 * j + 3] += b.w;
-              }
-            }
-            if constexpr (EPI == B200_EPI_BIAS_GELU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = gelu_tanh(f[j]);
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 o;
-              o.x = pack2<BF16>(f[8 * j + 0], f[8 * j + 1]);
-              o.y = pack2<BF16>(f[8 * j + 2], f[8 * j + 3]);
-              o.z = pack2<BF16>(f[8 * j + 4], f[8 * j + 5]);
-              o.w = pack2<BF16>(f[8 * j + 6], f[8 * j + 7]);
-              *reinterpret_cast<uint4*>(srow + (((hh * 4 + j) ^ (row_a & 7)) << 4)) = o;
-            }
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(bar_a) : "memory");   // staging tile complete
-          const int col = col0 + ch_b * 8;
-          if (col < p.N) {
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int rl = it * 16 + row_b0;
-              const int row = m0 + rl;
-              if (row < p.M) {
-                uint4 val = *reinterpret_cast<const uint4*>(buf + rl * 128 + ((ch_b ^ (rl & 7)) << 4));
-                if constexpr (EPI == B200_EPI_BIAS_MUL16) {   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
-                  const uint4 rs = __ldg(reinterpret_cast<const uint4*>(p.add16 + static_cast<size_t>(row) * p.N + col));
-                  const float2 a0 = unpack2<BF16>(val.x), a1 = unpack2<BF16>(val.y), a2 = unpack2<BF16>(val.z), a3 = unpack2<BF16>(val.w);
-                  const float2 r0 = unpack2<BF16>(rs.x), r1 = unpack2<BF16>(rs.y), r2 = unpack2<BF16>(rs.z), r3 = unpack2<BF16>(rs.w);
-                  val.x = pack2<BF16>(a0.x * r0.x, a0.y * r0.y);
-                  val.y = pack2<BF16>(a1.x * r1.x, a1.y * r1.y);
-                  val.z = pack2<BF16>(a2.x * r2.x, a2.y * r2.y);
-                  val.w = pack2<BF16>(a3.x * r3.x, a3.y * r3.y);
-                }
-                if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) {   // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
-                  const uint4 rs = __ldg(reinterpret_cast<const uint4*>(p.add16 + static_cast<size_t>(row) * p.N + col));
-                  const float2 a0 = unpack2<BF16>(val.x), a1 = unpack2<BF16>(val.y), a2 = unpack2<BF16>(val.z), a3 = unpack2<BF16>(val.w);
-                  const float2 r0 = unpack2<BF16>(rs.x), r1 = unpack2<BF16>(rs.y), r2 = unpack2<BF16>(rs.z), r3 = unpack2<BF16>(rs.w);
-                  val.x = pack2<BF16>(a0.x * gelu_tanh_grad(r0.x), a0.y * gelu_tanh_grad(r0.y));
-                  val.y = pack2<BF16>(a1.x * gelu_tanh_grad(r1.x), a1.y * gelu_tanh_grad(r1.y));
-                  val.z = pack2<BF16>(a2.x * gelu_tanh_grad(r2.x), a2.y * gelu_tanh_grad(r2.y));
-                  val.w = pack2<BF16>(a3.x * gelu_tanh_grad(r3.x), a3.y * gelu_tanh_grad(r3.y));
-                }
-                if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) {   // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
-                  const float2 a0 = unpack2<BF16>(val.x), a1 = unpack2<BF16>(val.y), a2 = unpack2<BF16>(val.z), a3 = unpack2<BF16>(val.w);
-                  uint4 gl;
-                  gl.x = pack2<BF16>(gelu_tanh(a0.x), gelu_tanh(a0.y));
-                  gl.y = pack2<BF16>(gelu_tanh(a1.x), gelu_tanh(a1.y));
-                  gl.z = pack2<BF16>(gelu_tanh(a2.x), gelu_tanh(a2.y));
-                  gl.w = pack2<BF16>(gelu_tanh(a3.x), gelu_tanh(a3.y));
-                  *reinterpret_cast<uint4*>(p.out16b + static_cast<size_t>(row) * p.N + col) = gl;
-                }
-                if constexpr (EPI == B200_EPI_BIAS_ADD16) {   // + shortcut, both already rounded to 16 bits like the reference
-                  const uint4 rs = __ldg(reinterpret_cast<const uint4*>(p.add16 + static_cast<size_t>(row) * p.N + col));
-                  const float2 a0 = unpack2<BF16>(val.x), a1 = unpack2<BF16>(val.y), a2 = unpack2<BF16>(val.z), a3 = unpack2<BF16>(val.w);
-                  const float2 r0 = unpack2<BF16>(rs.x), r1 = unpack2<BF16>(rs.y), r2 = unpack2<BF16>(rs.z), r3 = unpack2<BF16>(rs.w);
-                  val.x = pack2<BF16>(a0.x + r0.x, a0.y + r0.y);
-                  val.y = pack2<BF16>(a1.x + r1.x, a1.y + r1.y);
-                  val.z = pack2<BF16>(a2.x + r2.x, a2.y + r2.y);
-                  val.w = pack2<BF16>(a3.x + r3.x, a3.y + r3.y);
-                }
-                *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(row) * p.N + col) = val;
-              }
-            }
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(bar_b) : "memory");   // staging tile drained: safe to refill
         }
-        cc += NCH;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+        if (partial && kb1 < num_kb) {
+          __threadfence();                     // this segment's adds are visible ...
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+          if (te == 0) flag_release(flag, static_cast<unsigned long long>(kb1));   // ... the next segment may add
+        }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= p.M) continue;
+          uint32_t* orow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(row) * p.N);
+          const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j >= live) break;
+            const int col = n0 + 8 * j + 2 * cq;
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            if (p.bias) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              f0 += b.x; f1 += b.y;
+            }
+            if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+            uint32_t val = pack2<BF16>(f0, f1);
+            const size_t off = (static_cast<size_t>(row) * p.N + col) / 2;
+            if constexpr (EPI == B200_EPI_BIAS_MUL16) {   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
+              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+              val = pack2<BF16>(a.x * r.x, a.y * r.y);
+            }
+            if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) {   // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
+              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+              val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
+            }
+            if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) {   // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
+              const float2 a = unpack2<BF16>(val);
+              reinterpret_cast<uint32_t*>(p.out16b)[off] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
+            }
+            if constexpr (EPI == B200_EPI_BIAS_ADD16) {   // + shortcut, both already rounded to 16 bits like the reference
+              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+              val = pack2<BF16>(a.x + r.x, a.y + r.y);
+            }
+            orow[col / 2] = val;
+          }
+        }
       }
     }
   }
 
-  tc_fence_before();
   cluster_sync_all();   // the peer may still multicast into our smem / arrive on our barriers until it is done too
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
-  }
 }
 
 template <int BN, int EPI, bool BF16>
-int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmX, const GemmDev& p, int grid,
-               cudaStream_t stream) {
+int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t stream) {
   using C = Cfg<BN, EPI>;
   auto kern = gemm_kernel<BN, EPI, BF16>;
   B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tmA, tmB, tmX, p));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tmA, tmB, p));
   return B200_OK;
 }
 
 template <int BN, bool BF16>
-int launch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmX, const GemmDev& p, int grid,
-               cudaStream_t s) {
+int launch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
   switch (epi) {
-    case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16>(tmA, tmB, tmX, p, grid, s);
-    case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16>(tmA, tmB, tmX, p, grid, s);
+    case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16>(tmA, tmB, p, grid, s);
+    case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16>(tmA, tmB, p, grid, s);
   }
   set_error("gemm: unknown epilogue %d", epi);
   return B200_ERR_UNSUPPORTED;
 }
 
 template <int BN>
-int launch_bn(int bf16, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmX, const GemmDev& p,
-              int grid, cudaStream_t s) {
-  return bf16 ? launch_epi<BN, true>(epi, tmA, tmB, tmX, p, grid, s) : launch_epi<BN, false>(epi, tmA, tmB, tmX, p, grid, s);
+int launch_bn(int bf16, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
+  return bf16 ? launch_epi<BN, true>(epi, tmA, tmB, p, grid, s) : launch_epi<BN, false>(epi, tmA, tmB, p, grid, s);
 }
 
 constexpr int kStreamKMinKb = 32;          // K / 64 below which the split costs more than the idle tail it removes
@@ -635,8 +445,8 @@ int streamk_min_kb() {
 
 
 int pick_block_n(int M, int N, int K, bool resid, int sms) {
-  // minimise waves x per-tile time.  The kernel is bound by L2->SM operand bytes, not MMA cycles, so a tile costs
-  // ~ (A bytes + W/2 bytes per k-block per CTA) = 128 + BN/2 rather than BN (measured: r01 microbench, profiles/).
+  // minimise waves x per-tile time.  A tile's cost is modelled by the operand bytes a CTA receives per k-block, A plus
+  // its multicast half of W: 128 + BN/2.
   // Where the last wave is streamed along K (residual epilogue, long K) there is no wave rounding.
   if (N <= 128) return 128;   // narrow outputs (e.g. the VAE's 3-channel conv_out padded to 32): smallest tile that covers N
   static const bool no_sk = env_int("B200_GEMM_NO_STREAMK", 0) != 0;
@@ -745,8 +555,8 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     if (block_n == 0) {
       block_n = pick_block_n(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, sms);
       if (block_n == 192) block_n = (a.N % 256 == 0 || a.N > 1024) ? 256 : 128;     // W chunks are 64 wide per CTA: 128 or 256 only
-      // weight gradients: 256-wide tiles throughout -- the cost model's 128 for small outputs (proj: 1152 x 1152) measured slower
-      // once the tiles are split along K anyway (88.5 vs 75.4 us); B200_WGRAD_BN=128|256 forces a width for A/B runs
+      // weight gradients: 256-wide tiles for every output of at least 256 columns (the tiles are split along K anyway, so
+      // the wider tile only halves the A traffic); B200_WGRAD_BN=128|256 forces a width for A/B runs
       static const int wgrad_bn = env_int("B200_WGRAD_BN", 0);
       if (a.mn_major == 3) block_n = (wgrad_bn == 128 || wgrad_bn == 256) ? wgrad_bn : (a.N >= 256 ? 256 : block_n);
     }
@@ -754,7 +564,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   const GemmPlan plan = plan_gemm(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, a.mn_major == 3);
   const int bn = plan.bn;
 
-  CUtensorMap tmA, tmB, tmX;
+  CUtensorMap tmA, tmB;
   int conv_bw = 0, conv_bh = 0;
   {
     if (a.conv_taps > 0) {
@@ -793,14 +603,6 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
       const uint32_t boxB[2] = {BK, static_cast<uint32_t>(bn / 2)};   // each CTA of the pair fetches half and multicasts it
       B200_TRY(make_tmap_16bit(&tmB, a.W, 2, dimsB, strB, boxB, TMAP_SW_128));
     }
-    if (resid) {
-      const uint64_t dimsX[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
-      const uint64_t strX[1] = {static_cast<uint64_t>(a.N) * 4};
-      const uint32_t boxX[2] = {32, BM};
-      B200_TRY(make_tmap(&tmX, a.resid, 4, 2, dimsX, strX, boxX, TMAP_SW_128));
-    } else {
-      tmX = tmA;  // unused
-    }
   }
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
@@ -820,10 +622,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   p.conv_cblk = a.conv_taps > 0 ? a.conv_c / BK : 0;
   p.conv_h = a.conv_h; p.conv_w = a.conv_w; p.conv_bw = conv_bw; p.conv_bh = conv_bh;
   for (int i = 0; i < 9; ++i) { p.conv_dx[i] = a.conv_dx[i]; p.conv_dy[i] = a.conv_dy[i]; p.conv_dz[i] = a.conv_dz[i]; }
-  static const int dbg = env_int("B200_GEMM_DBG", 0);
-  p.dbg = dbg;
-  static const int no_wprefetch = env_int("B200_GEMM_NO_WPREFETCH", 0);     // A/B switch
-  p.w_const = (a.w_const && !no_wprefetch && a.conv_taps == 0 && !a.mn_major) ? 1 : 0;
+  p.resid = a.resid;
   p.mn_major = a.mn_major;
   const int pair_tiles = plan.pair_tiles;
   const int grid = 2 * plan.pairs;
@@ -838,9 +637,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     p.sk_flags = p.streamk ? a.sk_flags : nullptr;
   }
   switch (bn) {
-    case 128: return launch_bn<128>(a.bf16, a.epilogue, tmA, tmB, tmX, p, grid, stream);
-    case 192: return launch_bn<192>(a.bf16, a.epilogue, tmA, tmB, tmX, p, grid, stream);
-    default: return launch_bn<256>(a.bf16, a.epilogue, tmA, tmB, tmX, p, grid, stream);
+    case 128: return launch_bn<128>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
+    case 192: return launch_bn<192>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
+    default: return launch_bn<256>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
   }
 }
 

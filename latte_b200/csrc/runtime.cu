@@ -176,8 +176,8 @@ int device_sm_count(int* out) {
 int check_arch() {
   DevInfo d;
   B200_TRY(dev_info(&d));
-  B200_REQUIRE(d.major == 10, B200_ERR_ARCH, "latte_b200 kernels are sm_100a only; current device is sm_%d%d", d.major,
-               d.minor);
+  B200_REQUIRE(d.major == 9 && d.minor == 0, B200_ERR_ARCH, "latte_b200 kernels are sm_90a (Hopper) only; current device is sm_%d%d",
+               d.major, d.minor);
   return B200_OK;
 }
 

@@ -1,5 +1,5 @@
 // Backward-pass kernels of the training step (BASELINE config 5; reference train.py:206-222 -> autograd over models/latte.py).
-// Every GEMM of the backward (dgrad, wgrad) runs on the tcgen05 kernel of gemm.cu; this file holds what surrounds them:
+// Every GEMM of the backward (dgrad, wgrad) runs on the wgmma kernel of gemm.cu; this file holds what surrounds them:
 //   transpose16 / cast_transpose   16-bit [R,C] -> [C,R] operands for wgrad (K = tokens must be the contiguous dimension)
 //   gate_residual                  x_out = x + gate[b] * m (+ temp_embed row)          forward of latte.py:179-180 residuals
 //   gelu_fwd / gelu_bwd            tanh-GELU and its derivative, bias gradient (column sums) fused      (latte.py:169-171)
@@ -1250,7 +1250,7 @@ int launch_cast_transpose(const float* in, void* out16, void* out16_t, int rows,
 int launch_multi_cast(const void* table, int n_entries, long long total_chunks, int bf16, cudaStream_t stream) {
   B200_REQUIRE(table != nullptr && n_entries > 0 && total_chunks > 0, B200_ERR_SHAPE, "multi_cast: empty table");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(table) & 7) == 0, B200_ERR_ALIGN, "multi_cast: table must be 8-byte aligned");
-  const int blocks = static_cast<int>(total_chunks < 148 * 8 ? total_chunks : 148 * 8);
+  const int blocks = static_cast<int>(total_chunks < 132 * 8 ? total_chunks : 132 * 8);
   const MultiCastEntry* tab = static_cast<const MultiCastEntry*>(table);
   if (bf16) multi_cast_kernel<true><<<blocks, 256, 0, stream>>>(tab, n_entries, total_chunks);
   else multi_cast_kernel<false><<<blocks, 256, 0, stream>>>(tab, n_entries, total_chunks);
@@ -1265,7 +1265,7 @@ int launch_multi_tensor(const void* table, int n_entries, long long total_chunks
   B200_REQUIRE(op == MT_SUMSQ || op == MT_SCALE || op == MT_AXPBY, B200_ERR_UNSUPPORTED, "multi_tensor: op %d unknown", op);
   B200_REQUIRE(op != MT_SUMSQ || (accum != nullptr && (reinterpret_cast<uintptr_t>(accum) & 7) == 0), B200_ERR_ALIGN, "multi_tensor: accum missing");
   B200_REQUIRE(op != MT_SCALE || scalar != nullptr, B200_ERR_SHAPE, "multi_tensor: scalar missing");
-  const int blocks = static_cast<int>(total_chunks < 148 * 8 ? total_chunks : 148 * 8);
+  const int blocks = static_cast<int>(total_chunks < 132 * 8 ? total_chunks : 132 * 8);
   const MultiTensorEntry* tab = static_cast<const MultiTensorEntry*>(table);
   if (op == MT_SUMSQ) multi_tensor_kernel<MT_SUMSQ><<<blocks, 256, 0, stream>>>(tab, n_entries, total_chunks, a, b, scalar, accum);
   else if (op == MT_SCALE) multi_tensor_kernel<MT_SCALE><<<blocks, 256, 0, stream>>>(tab, n_entries, total_chunks, a, b, scalar, accum);
@@ -1281,7 +1281,7 @@ int launch_gate_residual(const float* x, const void* m16, const float* gate, lon
   B200_REQUIRE(ALIGNED16(x) && ALIGNED16(gate) && ALIGNED16(out) && (reinterpret_cast<uintptr_t>(m16) & 7) == 0 &&
                    (row_add == nullptr || ALIGNED16(row_add)), B200_ERR_ALIGN, "gate_residual: misaligned pointer");
   const long long total = static_cast<long long>(rows) * (dim / 4);
-  const int blocks = grid_for(total, 256, 148 * 16);
+  const int blocks = grid_for(total, 256, 132 * 16);
   const uint16_t* m = static_cast<const uint16_t*>(m16);
   if (bf16) gate_residual_kernel<true><<<blocks, 256, 0, stream>>>(x, m, gate, gate_bs, rows_per_batch, row_add, tokens, frames, out, rows, dim);
   else gate_residual_kernel<false><<<blocks, 256, 0, stream>>>(x, m, gate, gate_bs, rows_per_batch, row_add, tokens, frames, out, rows, dim);
@@ -1294,7 +1294,7 @@ static int grl_launch(cudaStream_t stream, const float* x, const uint16_t* m, co
                       const float* scale, long long mod_bs, int rpb, const float* row_add, int tokens, int frames, float* x_out, uint16_t* h,
                       int rows, int dim) {
   static const int minb = env_int("B200_GRL_MINB", 5);     // A/B switch: register cap (5 blocks of 4 warps per SM: 96 registers) vs none (134)
-  const int blocks = rows / 4 < 148 * 8 ? (rows + 3) / 4 : 148 * 8;
+  const int blocks = rows / 4 < 132 * 8 ? (rows + 3) / 4 : 132 * 8;
   if (minb >= 5) gate_residual_ln_kernel<BF16, NV, 5><<<blocks, 128, 0, stream>>>(x, m, gate, gate_bs, shift, scale, mod_bs, rpb, row_add, tokens, frames, x_out, h, rows, dim);
   else gate_residual_ln_kernel<BF16, NV, 1><<<blocks, 128, 0, stream>>>(x, m, gate, gate_bs, shift, scale, mod_bs, rpb, row_add, tokens, frames, x_out, h, rows, dim);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -1329,7 +1329,7 @@ int launch_gate_residual_ln(const float* x, const void* m16, const float* gate, 
 int launch_gelu_fwd(const void* u16, void* a16, long long n, int bf16, cudaStream_t stream) {
   B200_REQUIRE(n > 0 && n % 8 == 0, B200_ERR_SHAPE, "gelu: element count %lld must be a multiple of 8", n);
   B200_REQUIRE(ALIGNED16(u16) && ALIGNED16(a16), B200_ERR_ALIGN, "gelu: pointers must be 16-byte aligned");
-  const int blocks = grid_for(n / 8, 256, 148 * 16);
+  const int blocks = grid_for(n / 8, 256, 132 * 16);
   if (bf16) gelu_fwd_kernel<true><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(u16), static_cast<uint16_t*>(a16), n / 8);
   else gelu_fwd_kernel<false><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(u16), static_cast<uint16_t*>(a16), n / 8);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -1485,7 +1485,7 @@ int launch_ada_outer(const float* dmod, long long dmod_bs, const void* sc16, flo
   B200_REQUIRE(ALIGNED16(dW), B200_ERR_ALIGN, "ada_outer: dW must be 16-byte aligned");
   const size_t smem = static_cast<size_t>(batch) * dim * sizeof(float);
   B200_REQUIRE(smem <= 48 * 1024, B200_ERR_UNSUPPORTED, "ada_outer: batch * dim too large for the staging buffer");
-  const int blocks = NA < 148 * 8 ? NA : 148 * 8;
+  const int blocks = NA < 132 * 8 ? NA : 132 * 8;
   if (bf16) ada_outer_kernel<true><<<blocks, 256, smem, stream>>>(dmod, dmod_bs, static_cast<const uint16_t*>(sc16), dW, batch, NA, dim);
   else ada_outer_kernel<false><<<blocks, 256, smem, stream>>>(dmod, dmod_bs, static_cast<const uint16_t*>(sc16), dW, batch, NA, dim);
   B200_CHECK_CUDA(cudaGetLastError());

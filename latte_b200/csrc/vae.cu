@@ -1,5 +1,5 @@
 // AutoencoderKL.decode (diffusers 0.24.0 `Decoder`, called at reference sample/sample.py:114, sample_ddp.py:167,
-// pipeline_latte.py:758,771) as a chain of TMA implicit-GEMM convolutions on the tcgen05 GEMM kernel plus the
+// pipeline_latte.py:758,771) as a chain of TMA implicit-GEMM convolutions on the wgmma GEMM kernel plus the
 // memory-bound passes between them.  Activations are NHWC 16-bit so a pixel's channels are the GEMM K dimension.
 //   3x3 conv          -> launch_gemm in conv mode: 9 taps x (Cin/64) k-blocks, the A tile of a tap is the output tile's
 //                        pixel patch shifted by (dx, dy), borders zero-filled by TMA; bias (+ shortcut) in the epilogue
@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(256) moments_kernel(const uint16_t* __restrict
   }
 }
 
-inline int grid_for(long long n, int cap = 148 * 16) {
+inline int grid_for(long long n, int cap = 132 * 16) {
   long long b = (n + 255) / 256;
   return static_cast<int>(b < cap ? (b > 0 ? b : 1) : cap);
 }

@@ -1,4 +1,4 @@
-"""`Latte` — the reference's denoiser module surface, backed by hand-written sm_100a CUDA.
+"""`Latte` — the reference's denoiser module surface, backed by hand-written sm_90a CUDA.
 
 Mirrors the public interface of Vchitect/Latte `models/latte.py`:
   * constructor signature and attribute names                       (latte.py:208-232)
@@ -279,7 +279,7 @@ class Latte(DeviceCacheMixin, nn.Module):
 
     def _run(self, x, t, y, use_cfg, cfg_scale, trajectory_step=None):
         if not x.is_cuda:
-            raise RuntimeError("latte_b200.Latte runs on CUDA (sm_100a) only; there is no CPU fallback "
+            raise RuntimeError("latte_b200.Latte runs on CUDA (sm_90a) only; there is no CPU fallback "
                                "(the CPU truth lives in oracle/, which is test infrastructure)")
         if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
             if use_cfg or trajectory_step is not None:
@@ -443,7 +443,7 @@ class Latte(DeviceCacheMixin, nn.Module):
         lib = _lib.load()
         dev = self.pos_embed.device
         if dev.type != "cuda":
-            raise RuntimeError("latte_b200.Latte runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("latte_b200.Latte runs on CUDA (sm_90a) only; there is no CPU fallback")
         steps, B = timesteps.shape
         with torch.cuda.device(dev):
             shape, w, _, _ = self._pack()

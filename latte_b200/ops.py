@@ -33,7 +33,7 @@ def _sk_flags(device):
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("latte_b200.ops run on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("latte_b200.ops run on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 def linear(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, gelu: bool = False,

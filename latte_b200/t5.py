@@ -1,7 +1,7 @@
 """`T5EncoderModel` — the text encoder surface the reference's pipeline calls (`sample/pipeline_latte.py:214`:
 `self.text_encoder(input_ids, attention_mask=mask)[0]`, transformers' T5EncoderModel for t5-v1_1-xxl), backed by the same
-sm_100a kernels as the denoiser through ONE C-ABI call (`b200_t5_encode`): tcgen05 GEMMs (q|k|v in one, gated-GELU
-feed-forward with the multiply in the second GEMM's epilogue, fp32 residual adds as TMA reductions), the v3 attention
+sm_90a kernels as the denoiser through ONE C-ABI call (`b200_t5_encode`): wgmma GEMMs (q|k|v in one, gated-GELU
+feed-forward with the multiply in the second GEMM's epilogue, fp32 residual adds in the GEMM epilogue), the attention
 kernel with T5's relative-position bias and the prompt mask as additive score biases, RMSNorm and the embedding gather.
 
 Parameter names follow transformers' state dict (`shared.weight`, `encoder.block.N.layer.0.SelfAttention.q.weight`, ...),
@@ -180,7 +180,7 @@ class T5EncoderModel(DeviceCacheMixin, nn.Module):
     def forward(self, input_ids=None, attention_mask=None, return_dict=True, **unused):
         """input_ids (B, L <= 128) int64, attention_mask (B, L) 1 = keep -> last_hidden_state (B, L, d_model)."""
         if input_ids is None or not input_ids.is_cuda:
-            raise RuntimeError("latte_b200.T5EncoderModel runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("latte_b200.T5EncoderModel runs on CUDA (sm_90a) only; there is no CPU fallback")
         B, L = input_ids.shape
         if L > MAX_LEN:
             raise NotImplementedError(f"sequences longer than {MAX_LEN} tokens are not built (the pipeline uses 120)")

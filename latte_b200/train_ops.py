@@ -1,5 +1,5 @@
 """Native backend of latte_b200.training.TrainEngine: every op is one C-ABI call into liblatte_b200.so (csrc/train.cu for the
-backward passes, the tcgen05 GEMM / attention / LayerNorm kernels of the sampling path for the rest).  CUDA only — a CPU tensor
+backward passes, the wgmma GEMM / attention / LayerNorm kernels of the sampling path for the rest).  CUDA only — a CPU tensor
 raises; the torch restatement of the same ops lives in oracle/train_ops_oracle.py and is test infrastructure."""
 from __future__ import annotations
 
@@ -32,7 +32,7 @@ class NativeOps:
     def _cuda(*ts):
         for t in ts:
             if t is not None and not t.is_cuda:
-                raise RuntimeError("latte_b200 training ops run on CUDA (sm_100a) only; there is no CPU fallback")
+                raise RuntimeError("latte_b200 training ops run on CUDA (sm_90a) only; there is no CPU fallback")
 
     # ------------------------------------------------------------------ forward ops
     def ln_modulate(self, x, shift, scale, rpb):

@@ -2,7 +2,7 @@
 
 The reference trains through torch autograd over ~1000 eager kernels per forward.  Here the forward keeps the activations the
 backward needs and the backward is written out explicitly, op by op, over the same hand-written kernels as the sampling path
-(the tcgen05 GEMM does every dgrad and wgrad; wgrads accumulate in fp32 straight into the gradient buffers through the
+(the wgmma GEMM does every dgrad and wgrad; wgrads accumulate in fp32 straight into the gradient buffers through the
 residual epilogue) plus the kernels of csrc/train.cu (LayerNorm-modulate backward, gate / GELU backward with the bias and
 per-sample reductions fused, attention backward on tensor cores, 16-bit transposes, adaLN outer products).
 

@@ -1,6 +1,6 @@
 """`AutoencoderKL` — the decode half of the SD-VAE the reference samplers call once after the loop
 (`vae.decode(samples / 0.18215).sample`, sample/sample.py:114, sample_ddp.py:167, pipeline_latte.py:758,771), backed by
-TMA implicit-GEMM convolutions on the tcgen05 GEMM kernel (`b200_vae_decode`), and the encode half train.py calls on every
+TMA implicit-GEMM convolutions on the wgmma GEMM kernel (`b200_vae_decode`), and the encode half train.py calls on every
 batch (`vae.encode(x).latent_dist.sample()`, train.py:206-211; `b200_vae_encode`, SURVEY.md §8(f) rank 4).  Parameter names
 follow the diffusers 0.24.0 `AutoencoderKL` state dict (encoder.*, quant_conv.*, post_quant_conv.*, decoder.*), so
 `vae/diffusion_pytorch_model.safetensors` loads unchanged.  **Parity unpinned** (diffusers absent offline).  No CPU path."""
@@ -333,7 +333,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
         if self._temporal:
             raise NotImplementedError("AutoencoderKLTemporalDecoder.encode is outside the built path (the pipelines only decode with it)")
         if not x.is_cuda:
-            raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_90a) only; there is no CPU fallback")
         lib = _lib.load()
         dev = x.device
         n, ci, h, w = x.shape
@@ -453,7 +453,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
         """z (n, latent_channels, h, w) -> DecoderOutput(sample=(n, 3, 8h, 8w)).  `num_frames` is ignored by AutoencoderKL
         and required by AutoencoderKLTemporalDecoder (one clip per call: n == num_frames, as pipeline_latte.py:785-792 does)."""
         if not z.is_cuda:
-            raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_90a) only; there is no CPU fallback")
         lib = _lib.load()
         dev = z.device
         n, cz, h, w = z.shape

@@ -221,7 +221,7 @@ def t2v_forward(sd, cfg: T2VConfig, x, t, text, dtype=torch.float32, enable_temp
 
 
 def gemm_flops_per_video(cfg: T2VConfig, text_len: int) -> float:
-    """The Linear-layer part of `algorithmic_flops_per_video` (everything the tcgen05 GEMM kernel executes)."""
+    """The Linear-layer part of `algorithmic_flops_per_video` (everything the wgmma GEMM kernel executes)."""
     D, N, Fr, L = cfg.inner_dim, cfg.num_patches, cfg.video_length, cfg.num_layers
     T = N * Fr
     sp_lin = 2.0 * T * (3 * D * D + D * D + 2 * D * D + 8 * D * D)

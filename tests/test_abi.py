@@ -36,8 +36,8 @@ def test_no_libcuda_dependency():
     assert "libcuda.so" not in out and "libtorch" not in out and "libc10" not in out, out
 
 
-def test_sass_is_blackwell_native():
-    """The shipped cubin must contain tcgen05 MMA / TMEM / TMA instructions (UTC*MMA, LDTM, UTMALDG) and be sm_100a."""
+def test_sass_is_hopper_native():
+    """The shipped cubin must be sm_90a and contain warpgroup MMA and TMA instructions (HGMMA, UTMALDG)."""
     import shutil
     import subprocess
     from latte_b200 import _lib
@@ -45,16 +45,16 @@ def test_sass_is_blackwell_native():
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _lib.lib_path()], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    assert re.search(r"UTC\w*MMA", sass), "no tcgen05.mma in SASS"
-    assert "LDTM" in sass and "UTMALDG" in sass
+    assert "sm_90a" in sass
+    assert "HGMMA" in sass, "no wgmma in SASS"
+    assert "UTMALDG" in sass
     # Legacy mma.sync (HMMA) is allowed in exactly one place: the attention BACKWARD of the training step (csrc/train.cu,
     # ~2 % of the backward FLOPs, first version on register fragments).  Every forward / sampling kernel and every GEMM of the
-    # backward must be tcgen05.
+    # backward must be wgmma.
     legacy = set()
     for chunk in sass.split("Function : ")[1:]:
         name = chunk.split("\n", 1)[0]
-        if re.search(r"(?<!UTC)HMMA", chunk):
+        if re.search(r"(?<!G)HMMA", chunk):
             legacy.add(name)
     assert all("attn_bwd" in n for n in legacy), f"legacy mma.sync outside the attention backward: {sorted(legacy)[:4]}"
 

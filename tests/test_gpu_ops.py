@@ -107,8 +107,8 @@ def _attn_ref(qkv, batch, frames, tokens, heads, temporal):
 
 @pytest.fixture(params=[2, 3], ids=["attn_v2", "attn_v3"])
 def attn_impl(request):
-    """Both attention kernels serve the same contract (include/latte_b200.h: b200_set_attention_impl); every attention
-    test runs against each, whichever is the library default."""
+    """Every attention test runs through b200_set_attention_impl (include/latte_b200.h) with both non-default values the ABI
+    accepts; the sm_90a build has one attention kernel, so both select it -- the switch must keep accepting them."""
     from latte_b200 import _lib
     lib = _lib.load()
     _lib.check(lib.b200_set_attention_impl(request.param), "b200_set_attention_impl")

@@ -75,7 +75,7 @@ def test_linear_accum_small_and_wgrad_shapes(dev, dt):
 
 @pytest.mark.parametrize("dt", DTS)
 def test_wgrad_reads_untransposed_operands(dev, dt):
-    """dW += dY^T X with both activations as they lie in memory (the GEMM's MN-major UMMA descriptors, 64-wide chunk loads):
+    """dW += dY^T X with both activations as they lie in memory (the GEMM's MN-major wgmma descriptors, 64-wide block loads):
     full tiles, the half-width edge tile (n_in = 1152 = 4.5 x 256), ragged n_out (32, 1152 = 4.5 x 256 rows), stream-K."""
     nat, ref = _ops(dt)
     g = torch.Generator().manual_seed(7)
@@ -93,7 +93,7 @@ def test_wgrad_reads_untransposed_operands(dev, dt):
 
 @pytest.mark.parametrize("dt", DTS)
 def test_dgrad_reads_the_weight_in_place(dev, dt):
-    """dX = dY W with W in its nn.Linear [out, in] layout: A K-major, W through an MN-major UMMA descriptor (no W^T copy);
+    """dX = dY W with W in its nn.Linear [out, in] layout: A K-major, W through an MN-major wgmma descriptor (no W^T copy);
     n_in = 576 takes the explicit-transpose fallback."""
     nat, ref = _ops(dt)
     g = torch.Generator().manual_seed(8)

