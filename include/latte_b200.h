@@ -287,6 +287,37 @@ B200_API size_t b200_vae_encode_workspace_bytes(const B200VaeEncoder* e, int n_i
 B200_API int b200_vae_encode(const B200VaeEncoder* e, const float* x, int n_img, int h, int w, float* moments, void* workspace,
                              size_t workspace_bytes, void* stream);
 
+/* ---- single VAE layers, through the same internal launches b200_vae_decode / b200_vae_encode use (for op-level tests and
+ * for callers that assemble their own VAE).  Activations are NHWC 16-bit in `dtype`; weights are packed as by the host
+ * packers in latte_b200/vae.py; bias fp32 [cout] or NULL.
+ * b200_vae_conv, `kind`:
+ *   B200_VAE_CONV3X3     Conv2d 3x3, padding 1: x [n_img, h, w, cin] -> out16 [n_img, h, w, cout]; w16 [cout][ky*3+kx][cin].
+ *                        w >= 128: w % 128 == 0; w < 128: 128 % w == 0 and h % (128 / w) == 0.
+ *   B200_VAE_CONV_T3     Conv3d (3,1,1), padding (1,0,0) over the n_img frames of ONE clip (zero padding at both ends):
+ *                        cin == cout, w16 [cout][kt][cin]; same tiling rule.
+ *   B200_VAE_CONV_DOWN2  Downsample2D: F.pad (0,1,0,1) then Conv2d 3x3 stride 2 on an h x w input (h, w even): out16
+ *                        [n_img, h/2, w/2, cout]; w16 [cout][tap = oy*2+ox][phase = py*2+px][cin]; scratch receives the
+ *                        space-to-depth input, n_img * h * w * cin 16-bit values.  add16 must be NULL.
+ * add16: NULL or [n_img, h, w, cout] 16-bit, added after the 16-bit rounding of conv + bias (the resnet "+ shortcut").
+ * cin % 64 == 0, cout % 32 == 0; x, out16, add16, scratch 16-byte aligned.                                              */
+enum { B200_VAE_CONV3X3 = 0, B200_VAE_CONV_T3 = 1, B200_VAE_CONV_DOWN2 = 2 };
+B200_API int b200_vae_conv(const void* x, const void* w16, const float* bias, const void* add16, void* out16, void* scratch, int n_img,
+                           int h, int w, int cin, int cout, int kind, int dtype, void* stream);
+/* GroupNorm(groups, C, eps) (+ SiLU when silu != 0) over each of n_img images of hw pixels: x, y [n_img, hw, C] 16-bit;
+ * gamma, beta fp32 [C]; part: n_img * groups * 2 floats of scratch.  C / groups must be 4 or a multiple of 8, C / 8 must
+ * divide 256.  The temporal decoder's GroupNorm over a clip is one image of frames * hw pixels.                         */
+B200_API int b200_group_norm(const void* x, void* y, const float* gamma, const float* beta, float* part, int n_img, int hw, int C,
+                             int groups, float eps, int silu, int dtype, void* stream);
+/* Mid-block attention of the VAE (one head over the h*w pixels of each image):
+ * out = x + to_out(softmax(q k^T / sqrt(C)) v) with q, k, v projections of GroupNorm(groups, C, eps)(x).
+ * x, out [n_img, h*w, C] 16-bit; *_w16 [C, C] 16-bit nn.Linear weights; o_b = to_out bias + to_out weight . to_v bias (the
+ * v bias folded in, latte_b200/vae.py fold_v_bias).  C % 64 == 0, (h*w) % 64 == 0; workspace 1024-byte aligned.          */
+B200_API size_t b200_vae_mid_attention_workspace_bytes(int n_img, int h, int w, int C, int groups);
+B200_API int b200_vae_mid_attention(const void* x, void* out, const float* gn_g, const float* gn_b, const void* q_w16, const float* q_b,
+                                    const void* k_w16, const float* k_b, const void* v_w16, const void* o_w16, const float* o_b, int n_img,
+                                    int h, int w, int C, int groups, float eps, int dtype, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+
 /* Thread-local description of the last failure on this thread ("" if none). */
 B200_API const char* b200_last_error(void);
 B200_API int b200_abi_version(void);

@@ -15,6 +15,7 @@ GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buff
 OK = 0
 FP16, BF16 = 0, 1
 EPI_BIAS, EPI_BIAS_GELU, EPI_GATE_RESIDUAL, EPI_BIAS_ADD16, EPI_BIAS_MUL16, EPI_BIAS_GELU_BOTH, EPI_MUL_GELUGRAD16 = 0, 1, 2, 3, 4, 5, 6
+VAE_CONV3X3, VAE_CONV_T3, VAE_CONV_DOWN2 = 0, 1, 2
 ERR_NAMES = {-1: "SHAPE", -2: "DTYPE", -3: "ALIGN", -4: "ARCH", -5: "WORKSPACE", -6: "CUDA", -7: "UNSUPPORTED"}
 
 
@@ -140,6 +141,14 @@ EXPORTS = {
                                   C.c_void_p]),
     "b200_vae_decode_temporal": (C.c_int, [C.POINTER(VaeDecoder), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                            C.c_size_t, C.c_void_p]),
+    "b200_vae_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b200_group_norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_float, C.c_int, C.c_int, C.c_void_p]),
+    "b200_vae_mid_attention_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b200_vae_mid_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                         C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200_sampler_step": (C.c_int, [C.POINTER(SamplerTables), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p]),

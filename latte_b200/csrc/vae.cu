@@ -3,7 +3,7 @@
 // memory-bound passes between them.  Activations are NHWC 16-bit so a pixel's channels are the GEMM K dimension.
 //   3x3 conv          -> launch_gemm in conv mode: 9 taps x (Cin/64) k-blocks, the A tile of a tap is the output tile's
 //                        pixel patch shifted by (dx, dy), borders zero-filled by TMA; bias (+ shortcut) in the epilogue
-//   GroupNorm(32)+SiLU -> gn_stats (fp32 partial sums, fp64 combine) + gn_apply (one read, one write)
+//   GroupNorm(32)+SiLU -> gn_stats (fp32 partial sums of x - pivot, fp64 combine) + gn_apply (one read, one write)
 //   nearest 2x upsample, 1x1 convs (plain GEMM), mid-block attention (three GEMMs + a row softmax), tiny first/last layers.
 // PARITY UNPINNED: diffusers is not available offline; the CPU truth is oracle/vae_oracle.py's restatement.
 #include "common.h"
@@ -16,7 +16,15 @@ namespace {
 // ---------------------------------------------------------------------------------- GroupNorm statistics
 // x: [n_img, hw, C] 16-bit.  One block handles `rows_per_block` pixels of one image; thread t owns 8 channels
 // (c8 = t % (C/8)); per-group partial (sum, sumsq) are reduced in smem and added to part[img][group][2] (fp32 atomics:
-// <= a few hundred adds per slot).
+// <= a few hundred adds per slot).  The sums are of x - pivot, pivot = the group's first value in the image (gn_pivot):
+// with |mean| >> std, E[x^2] - mean^2 of the raw values cancels most of the fp32 bits of the variance (at mean = 64 std
+// over 65536 pixels the fp16 outputs were off by up to 7 roundings); the shifted sums keep them, and a constant group
+// sums to exactly zero.
+template <bool BF16>
+__device__ __forceinline__ float gn_pivot(const uint16_t* x, int img, int hw, int C, int group, int cpg) {
+  return unpack2<BF16>(static_cast<uint32_t>(x[static_cast<size_t>(img) * hw * C + group * cpg])).x;
+}
+
 template <bool BF16>
 __global__ void __launch_bounds__(256) gn_stats_kernel(const uint16_t* __restrict__ x, float* __restrict__ part, int hw, int C,
                                                        int groups, int rows_per_block) {
@@ -30,11 +38,16 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const uint16_t* __restric
   const int rlane = threadIdx.x / c8n;
   const int rstep = blockDim.x / c8n;
   const int row0 = blockIdx.x * rows_per_block;
+  // pivots of this thread's channels 0-3 and 4-7 (two groups when cpg == 4)
+  const float p_lo = gn_pivot<BF16>(x, img, hw, C, (c8 * 8) / cpg, cpg);
+  const float p_hi = cpg == 4 ? gn_pivot<BF16>(x, img, hw, C, (c8 * 8) / cpg + 1, cpg) : p_lo;
   float s = 0.f, q = 0.f;
   float s2 = 0.f, q2 = 0.f;             // second group when 8 channels straddle two groups (cpg == 4)
   for (int r = row0 + rlane; r < row0 + rows_per_block && r < hw; r += rstep) {
     const uint4 v = *reinterpret_cast<const uint4*>(x + (static_cast<size_t>(img) * hw + r) * C + c8 * 8);
-    const float2 a = unpack2<BF16>(v.x), b = unpack2<BF16>(v.y), c = unpack2<BF16>(v.z), d = unpack2<BF16>(v.w);
+    float2 a = unpack2<BF16>(v.x), b = unpack2<BF16>(v.y), c = unpack2<BF16>(v.z), d = unpack2<BF16>(v.w);
+    a.x -= p_lo; a.y -= p_lo; b.x -= p_lo; b.y -= p_lo;
+    c.x -= p_hi; c.y -= p_hi; d.x -= p_hi; d.y -= p_hi;
     if (cpg >= 8) {
       s += (a.x + a.y) + (b.x + b.y) + (c.x + c.y) + (d.x + d.y);
       q += (a.x * a.x + a.y * a.y) + (b.x * b.x + b.y * b.y) + (c.x * c.x + c.y * c.y) + (d.x * d.x + d.y * d.y);
@@ -60,13 +73,15 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const uint16_t* __restric
   for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) atomicAdd(&part[static_cast<size_t>(img) * groups * 2 + i], s_acc[i]);
 }
 
-// (sum, sumsq) -> (mean, rstd), combined in fp64 once per (image, group)
-__global__ void gn_finalize_kernel(float* __restrict__ part, int n_slots, double cnt, float eps) {
+// (sum, sumsq) of x - pivot -> (mean, rstd), combined in fp64 once per (image, group)
+template <bool BF16>
+__global__ void gn_finalize_kernel(float* __restrict__ part, const uint16_t* __restrict__ x, int n_slots, int groups, int hw, int C,
+                                   double cnt, float eps) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_slots) return;
-  const double m = static_cast<double>(part[2 * i]) / cnt;
+  const double m = static_cast<double>(part[2 * i]) / cnt;     // mean - pivot
   const double var = static_cast<double>(part[2 * i + 1]) / cnt - m * m;
-  part[2 * i] = static_cast<float>(m);
+  part[2 * i] = static_cast<float>(gn_pivot<BF16>(x, i / groups, hw, C, i % groups, C / groups) + m);
   part[2 * i + 1] = rsqrtf(static_cast<float>(var > 0.0 ? var : 0.0) + eps);
 }
 
@@ -301,11 +316,11 @@ int launch_gn(const void* x, float* part, const float* gamma, const float* beta,
   const double cnt = static_cast<double>(hw) * (C / groups);
   if (bf16) {
     gn_stats_kernel<true><<<grid, 256, smem, stream>>>(static_cast<const uint16_t*>(x), part, hw, C, groups, rows_per_block);
-    gn_finalize_kernel<<<(slots + 127) / 128, 128, 0, stream>>>(part, slots, cnt, eps);
+    gn_finalize_kernel<true><<<(slots + 127) / 128, 128, 0, stream>>>(part, static_cast<const uint16_t*>(x), slots, groups, hw, C, cnt, eps);
     gn_apply_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(x), part, gamma, beta, static_cast<uint16_t*>(y), hw, C, groups, rows_per_block, do_silu);
   } else {
     gn_stats_kernel<false><<<grid, 256, smem, stream>>>(static_cast<const uint16_t*>(x), part, hw, C, groups, rows_per_block);
-    gn_finalize_kernel<<<(slots + 127) / 128, 128, 0, stream>>>(part, slots, cnt, eps);
+    gn_finalize_kernel<false><<<(slots + 127) / 128, 128, 0, stream>>>(part, static_cast<const uint16_t*>(x), slots, groups, hw, C, cnt, eps);
     gn_apply_kernel<false><<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(x), part, gamma, beta, static_cast<uint16_t*>(y), hw, C, groups, rows_per_block, do_silu);
   }
   B200_CHECK_CUDA(cudaGetLastError());
@@ -460,6 +475,19 @@ int conv_t3(VaeCtx& c, const void* x, const void* w16, const float* bias, void* 
   a.epilogue = add16 ? B200_EPI_BIAS_ADD16 : B200_EPI_BIAS; a.out16 = y; a.add16 = add16;
   a.conv_taps = 3; a.conv_n = c.n_img; a.conv_h = h; a.conv_w = w; a.conv_c = ch;
   for (int t = 0; t < 9; ++t) { a.conv_dx[t] = 0; a.conv_dy[t] = 0; a.conv_dz[t] = t < 3 ? t - 1 : 0; }
+  return launch_gemm(a, c.stream);
+}
+
+// Downsample2D (pad (0,1,0,1), Conv2d 3x3 stride 2) on an h x w input: space_to_depth into `s2d` [n_img, h/2, w/2, 4 cin], then
+// the 2x2-tap implicit GEMM over 4 cin channels; w16 is [cout][tap = oy*2+ox][phase = py*2+px][cin] (host packer)
+int conv_down2(VaeCtx& c, const void* x, void* s2d, const void* w16, const float* bias, void* y, int h, int w, int cin, int cout) {
+  B200_TRY(launch_space_to_depth(x, s2d, c.n_img, h, w, cin, c.stream));
+  const int ho = h / 2, wo = w / 2;
+  GemmArgs a{};
+  a.A = s2d; a.W = w16; a.bias = bias; a.M = c.n_img * ho * wo; a.N = cout; a.K = 4 * 4 * cin; a.bf16 = c.bf16;
+  a.epilogue = B200_EPI_BIAS; a.out16 = y;
+  a.conv_taps = 4; a.conv_n = c.n_img; a.conv_h = ho; a.conv_w = wo; a.conv_c = 4 * cin;
+  for (int t = 0; t < 9; ++t) { a.conv_dx[t] = t < 4 ? (t & 1) : 0; a.conv_dy[t] = t < 4 ? (t >> 1) : 0; a.conv_dz[t] = 0; }
   return launch_gemm(a, c.stream);
 }
 
@@ -663,14 +691,8 @@ int vae_encode(const B200VaeEncoder* e, const float* x, int n_img, int h, int w,
       const int co = e->down_channels[b];
       int fr[3], nf = 0;
       for (int i = 0; i < 4; ++i) if (i != xi) fr[nf++] = i;
-      B200_TRY(launch_space_to_depth(c.ws.buf[xi], c.ws.buf[fr[0]], n_img, ch, cw, co, stream));
+      B200_TRY(conv_down2(c, c.ws.buf[xi], c.ws.buf[fr[0]], e->down_w16[b], e->down_b[b], c.ws.buf[fr[1]], ch, cw, co, co));
       ch /= 2; cw /= 2;
-      GemmArgs a{};
-      a.A = c.ws.buf[fr[0]]; a.W = e->down_w16[b]; a.bias = e->down_b[b]; a.M = n_img * ch * cw; a.N = co; a.K = 4 * 4 * co; a.bf16 = c.bf16;
-      a.epilogue = B200_EPI_BIAS; a.out16 = c.ws.buf[fr[1]];
-      a.conv_taps = 4; a.conv_n = n_img; a.conv_h = ch; a.conv_w = cw; a.conv_c = 4 * co;
-      for (int t = 0; t < 9; ++t) { a.conv_dx[t] = t < 4 ? (t & 1) : 0; a.conv_dy[t] = t < 4 ? (t >> 1) : 0; a.conv_dz[t] = 0; }
-      B200_TRY(launch_gemm(a, stream));
       xi = fr[1];
     }
   }
@@ -690,6 +712,39 @@ int vae_encode(const B200VaeEncoder* e, const float* x, int n_img, int h, int w,
   }
   return B200_OK;
 }
+
+// ====================================================================================================== single layers
+// The C-ABI entry points below run one layer of the decoder / encoder through the same internal functions, so each can be
+// compared with its torch op in isolation.
+int mid_attn_ok(int n_img, int h, int w, int C, int groups) {
+  B200_REQUIRE(n_img > 0 && h > 0 && w > 0 && C > 0 && groups > 0, B200_ERR_SHAPE, "vae attention: bad arguments");
+  B200_REQUIRE(C % 64 == 0 && C % groups == 0 && (h * w) % 64 == 0, B200_ERR_UNSUPPORTED,
+               "vae attention: C=%d must be a multiple of 64 and of groups=%d, h*w=%d a multiple of 64", C, groups, h * w);
+  return B200_OK;
+}
+
+// buf[0] = x (read only), buf[1] = the caller's output (also the GroupNorm result until the last GEMM), buf[2] = attention
+// output; then the scratch of mid_attention exactly as vae_carve lays it out
+void mid_attn_carve(int n_img, int hw, int C, int groups, void* base, VaeWs* ws) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    uint8_t* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
+    off += up1k(bytes);
+    return p;
+  };
+  const size_t act = static_cast<size_t>(n_img) * hw * C * 2;
+  ws->buf[2] = take(act);
+  ws->q = take(act);
+  ws->k = take(act);
+  ws->vt = take(static_cast<size_t>(C) * hw * 2);
+  ws->p16 = take(static_cast<size_t>(hw) * hw * 2);
+  ws->scores = reinterpret_cast<float*>(take(static_cast<size_t>(hw) * hw * 4));
+  ws->ones = reinterpret_cast<float*>(take(static_cast<size_t>(hw) * 4));
+  ws->part = reinterpret_cast<float*>(take(static_cast<size_t>(n_img) * groups * 2 * 4));
+  ws->bytes = off;
+}
+
+inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
 }  // namespace b200
@@ -724,6 +779,70 @@ B200_API int b200_vae_decode_temporal(const B200VaeDecoder* d, const float* z, i
                                       void* workspace, size_t workspace_bytes, void* stream) {
   B200_REQUIRE(num_frames > 0, B200_ERR_SHAPE, "vae: num_frames must be positive");
   return b200::vae_decode(d, z, n_img, h, w, num_frames, out, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+B200_API int b200_vae_conv(const void* x, const void* w16, const float* bias, const void* add16, void* out16, void* scratch, int n_img,
+                           int h, int w, int cin, int cout, int kind, int dtype, void* stream) {
+  using namespace b200;
+  B200_REQUIRE(n_img > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, B200_ERR_SHAPE, "vae conv: bad shape");
+  B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "vae conv: dtype %d", dtype);
+  B200_REQUIRE(kind == B200_VAE_CONV3X3 || kind == B200_VAE_CONV_T3 || kind == B200_VAE_CONV_DOWN2, B200_ERR_UNSUPPORTED,
+               "vae conv: unknown kind %d", kind);
+  B200_REQUIRE(cin % 64 == 0, B200_ERR_UNSUPPORTED, "vae conv: cin=%d must be a multiple of 64", cin);
+  B200_REQUIRE(kind != B200_VAE_CONV_T3 || cin == cout, B200_ERR_UNSUPPORTED, "vae conv: the temporal conv maps C -> C (cin %d, cout %d)", cin, cout);
+  B200_REQUIRE(kind != B200_VAE_CONV_DOWN2 || (add16 == nullptr && h % 2 == 0 && w % 2 == 0), B200_ERR_UNSUPPORTED,
+               "vae conv: the stride-2 conv takes an even-sized input and no shortcut");
+  B200_REQUIRE(x && w16 && out16 && al16(x) && al16(out16) && (kind != B200_VAE_CONV_DOWN2 || (scratch && al16(scratch))), B200_ERR_ALIGN,
+               "vae conv: x, out16 (and the stride-2 scratch) must be 16-byte aligned");
+  B200_TRY(check_arch());
+  VaeCtx c{};
+  c.n_img = n_img; c.bf16 = dtype == B200_BF16; c.stream = static_cast<cudaStream_t>(stream);
+  if (kind == B200_VAE_CONV3X3) return conv3x3(c, x, w16, bias, out16, h, w, cin, cout, add16);
+  if (kind == B200_VAE_CONV_T3) return conv_t3(c, x, w16, bias, out16, h, w, cin, add16);
+  return conv_down2(c, x, scratch, w16, bias, out16, h, w, cin, cout);
+}
+
+B200_API int b200_group_norm(const void* x, void* y, const float* gamma, const float* beta, float* part, int n_img, int hw, int C,
+                             int groups, float eps, int silu, int dtype, void* stream) {
+  using namespace b200;
+  B200_REQUIRE(n_img > 0 && n_img <= 65535 && hw > 0 && C > 0 && groups > 0, B200_ERR_SHAPE, "group norm: bad shape");
+  B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "group norm: dtype %d", dtype);
+  B200_REQUIRE(x && y && gamma && beta && part && al16(x) && al16(y) && (reinterpret_cast<uintptr_t>(part) & 7) == 0, B200_ERR_ALIGN,
+               "group norm: x and y must be 16-byte aligned, part 8-byte aligned");
+  B200_TRY(check_arch());
+  return launch_gn(x, part, gamma, beta, y, n_img, hw, C, groups, eps, silu, dtype == B200_BF16, static_cast<cudaStream_t>(stream));
+}
+
+B200_API size_t b200_vae_mid_attention_workspace_bytes(int n_img, int h, int w, int C, int groups) {
+  if (b200::mid_attn_ok(n_img, h, w, C, groups) != B200_OK) return 0;
+  b200::VaeWs ws;
+  b200::mid_attn_carve(n_img, h * w, C, groups, nullptr, &ws);
+  return ws.bytes;
+}
+
+B200_API int b200_vae_mid_attention(const void* x, void* out, const float* gn_g, const float* gn_b, const void* q_w16, const float* q_b,
+                                    const void* k_w16, const float* k_b, const void* v_w16, const void* o_w16, const float* o_b, int n_img,
+                                    int h, int w, int C, int groups, float eps, int dtype, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  using namespace b200;
+  B200_TRY(mid_attn_ok(n_img, h, w, C, groups));
+  B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "vae attention: dtype %d", dtype);
+  B200_REQUIRE(x && out && gn_g && gn_b && q_w16 && k_w16 && v_w16 && o_w16 && al16(x) && al16(out) && workspace &&
+                   (reinterpret_cast<uintptr_t>(workspace) & 1023) == 0,
+               B200_ERR_ALIGN, "vae attention: x and out must be 16-byte aligned, workspace 1024-byte aligned");
+  B200_TRY(check_arch());
+  VaeCtx c{};
+  c.n_img = n_img; c.bf16 = dtype == B200_BF16; c.stream = static_cast<cudaStream_t>(stream);
+  c.groups = groups; c.eps = eps; c.temporal_eps = eps;
+  mid_attn_carve(n_img, h * w, C, groups, workspace, &c.ws);
+  B200_REQUIRE(c.ws.bytes <= workspace_bytes, B200_ERR_WORKSPACE, "vae attention: workspace too small: need %zu bytes, got %zu",
+               c.ws.bytes, workspace_bytes);
+  c.ws.buf[0] = static_cast<uint8_t*>(const_cast<void*>(x));
+  c.ws.buf[1] = static_cast<uint8_t*>(out);
+  c.ws.buf[3] = nullptr;
+  const MidAttn at{gn_g, gn_b, q_w16, q_b, k_w16, k_b, v_w16, o_w16, o_b};
+  int out_idx;   // with the input in buf[0] the result lands in buf[1] = out
+  return mid_attention(c, at, C, 0, h, w, &out_idx);
 }
 
 }  // extern "C"

@@ -114,6 +114,69 @@ def cross_attention(q: torch.Tensor, kv: torch.Tensor, batch: int, q_rows_per_ba
     return out
 
 
+_VAE_CONV_KINDS = {"3x3": _lib.VAE_CONV3X3, "t3": _lib.VAE_CONV_T3, "down2": _lib.VAE_CONV_DOWN2}
+
+
+def vae_conv(x: torch.Tensor, w16: torch.Tensor, bias: torch.Tensor | None, kind: str = "3x3",
+             add16: torch.Tensor | None = None) -> torch.Tensor:
+    """One VAE convolution (b200_vae_conv).  x [n, h, w, cin] 16-bit NHWC; w16 the packed 2-D weight (vae.pack_conv3x3 /
+    pack_conv_t3 / pack_down2, cast to x's dtype); bias fp32 [cout]; add16 like the output.  kind "3x3": Conv2d padding 1;
+    "t3": Conv3d (3,1,1) over the n frames of one clip; "down2": pad (0,1,0,1) + stride-2 Conv2d -> [n, h/2, w/2, cout]."""
+    _need_cuda(x, w16, bias, add16)
+    assert x.dim() == 4 and x.is_contiguous() and w16.is_contiguous() and w16.dtype == x.dtype
+    n, h, w, cin = x.shape
+    cout = w16.shape[0]
+    ho, wo = (h // 2, w // 2) if kind == "down2" else (h, w)
+    out = torch.empty(n, ho, wo, cout, dtype=x.dtype, device=x.device)
+    if add16 is not None:
+        assert add16.shape == out.shape and add16.dtype == x.dtype and add16.is_contiguous()
+    scratch = torch.empty(n, ho, wo, 4 * cin, dtype=x.dtype, device=x.device) if kind == "down2" else None
+    with torch.cuda.device(x.device):
+        rc = _lib.load().b200_vae_conv(x.data_ptr(), w16.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                       add16.data_ptr() if add16 is not None else None, out.data_ptr(),
+                                       scratch.data_ptr() if scratch is not None else None, n, h, w, cin, cout,
+                                       _VAE_CONV_KINDS[kind], _dt(x), _stream(x))
+    _lib.check(rc, "b200_vae_conv")
+    return out
+
+
+def group_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float, silu: bool = False) -> torch.Tensor:
+    """GroupNorm (+ SiLU) of the VAE (b200_group_norm) over each image of x [n, ..., C] 16-bit channels-last; gamma, beta fp32 [C]."""
+    _need_cuda(x, gamma, beta)
+    assert x.is_contiguous() and gamma.dtype == beta.dtype == torch.float32
+    n, C = x.shape[0], x.shape[-1]
+    out = torch.empty_like(x)
+    part = torch.empty(n, groups, 2, dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        rc = _lib.load().b200_group_norm(x.data_ptr(), out.data_ptr(), gamma.data_ptr(), beta.data_ptr(), part.data_ptr(), n,
+                                         x.numel() // (n * C), C, groups, eps, int(silu), _dt(x), _stream(x))
+    _lib.check(rc, "b200_group_norm")
+    return out
+
+
+def vae_mid_attention(x: torch.Tensor, gn_g: torch.Tensor, gn_b: torch.Tensor, q_w16: torch.Tensor, q_b: torch.Tensor,
+                      k_w16: torch.Tensor, k_b: torch.Tensor, v_w16: torch.Tensor, o_w16: torch.Tensor, o_b: torch.Tensor,
+                      groups: int, eps: float = 1e-6) -> torch.Tensor:
+    """Mid-block attention of the VAE (b200_vae_mid_attention): x [n, h, w, C] 16-bit NHWC -> x + to_out(softmax(q k^T / sqrt(C)) v),
+    q/k/v of GroupNorm(x).  *_w16 [C, C] in x's dtype; biases fp32, o_b with the v bias folded in (vae.fold_v_bias)."""
+    _need_cuda(x, q_w16, k_w16, v_w16, o_w16)
+    assert x.dim() == 4 and x.is_contiguous() and all(t.is_contiguous() and t.dtype == x.dtype for t in (q_w16, k_w16, v_w16, o_w16))
+    n, h, w, C = x.shape
+    lib = _lib.load()
+    need = lib.b200_vae_mid_attention_workspace_bytes(n, h, w, C, groups)
+    if need == 0:
+        raise RuntimeError("b200_vae_mid_attention: unsupported shape: " + _lib.last_error())
+    ws = torch.empty(need + 1024, dtype=torch.uint8, device=x.device)
+    base = (ws.data_ptr() + 1023) // 1024 * 1024
+    out = torch.empty_like(x)
+    with torch.cuda.device(x.device):
+        rc = lib.b200_vae_mid_attention(x.data_ptr(), out.data_ptr(), gn_g.data_ptr(), gn_b.data_ptr(), q_w16.data_ptr(), q_b.data_ptr(),
+                                        k_w16.data_ptr(), k_b.data_ptr(), v_w16.data_ptr(), o_w16.data_ptr(), o_b.data_ptr(),
+                                        n, h, w, C, groups, eps, _dt(x), base, need, _stream(x))
+    _lib.check(rc, "b200_vae_mid_attention")
+    return out
+
+
 _U8_DT = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 

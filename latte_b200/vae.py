@@ -18,6 +18,41 @@ from . import _lib
 from ._cache import DeviceCacheMixin
 
 
+# ---- weight layouts of the native layers (the packers below and the op-level tests both use these) -------------------
+def pack_conv3x3(wt):
+    """Conv2d 3x3 weight OIHW -> [O][tap = ky*3+kx][I] as a 2-D [O, 9I] view (b200_vae_conv, B200_VAE_CONV3X3)."""
+    return wt.detach().permute(0, 2, 3, 1).reshape(wt.shape[0], -1)
+
+
+def pack_linear(wt):
+    """nn.Linear [O, I] or 1x1 Conv2d [O, I, 1, 1] weight -> [O, I]."""
+    return wt.detach().reshape(wt.shape[0], -1)
+
+
+def pack_conv_t3(wt, scale=1.0):
+    """Conv3d (3,1,1) weight [O][I][kt][1][1] -> fp32 [O][kt][I] as [O, 3I], times `scale` (B200_VAE_CONV_T3)."""
+    return (wt.detach().float() * scale).reshape(wt.shape[0], wt.shape[1], 3).permute(0, 2, 1).reshape(wt.shape[0], -1)
+
+
+def pack_down2(wt):
+    """Conv2d(C, C, 3, stride 2) after F.pad (0,1,0,1) -> 2x2-tap conv over the space-to-depth input: input pixel (2y+dy,
+    2x+dx) is phase (dy & 1, dx & 1) at offset (dy >> 1, dx >> 1); fp32 [O][tap = oy*2+ox][phase = py*2+px][I] as [O, 16I],
+    zeros at (phase 1, offset 1), which no 3x3 tap reaches (B200_VAE_CONV_DOWN2)."""
+    O, I = wt.shape[:2]
+    out = torch.zeros(O, 2, 2, 2, 2, I, dtype=torch.float32, device=wt.device)     # [O][oy][ox][py][px][I]
+    w = wt.detach().float()
+    for dy in range(3):
+        for dx in range(3):
+            out[:, dy >> 1, dx >> 1, dy & 1, dx & 1, :] = w[:, :, dy, dx]
+    return out.reshape(O, -1)
+
+
+def fold_v_bias(o_w, o_b, v_b):
+    """softmax rows sum to 1, so P (V + 1 b_v^T) W_o^T + b_o = P V W_o^T + (W_o b_v + b_o): the fp32 output bias of the
+    mid-block attention with the v bias folded in (b200_vae_mid_attention takes no v bias)."""
+    return o_b.detach().float() + o_w.detach().float() @ v_b.detach().float()
+
+
 class _Resnet(nn.Module):
     def __init__(self, cin, cout, groups):
         super().__init__()
@@ -270,19 +305,9 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             keep.append(t)
             return t.data_ptr()
 
-        conv16 = lambda wt: t16(wt.detach().permute(0, 2, 3, 1).reshape(wt.shape[0], -1))      # noqa: E731  OIHW -> [O][tap][I]
-        lin16 = lambda wt: t16(wt.detach().reshape(wt.shape[0], -1))                           # noqa: E731
-
-        def down16(wt):
-            """Conv2d(C, C, 3, stride 2) after F.pad (0,1,0,1) -> 2x2-tap conv over the space-to-depth input: input pixel (2y+dy,
-            2x+dx) is phase (dy & 1, dx & 1) at offset (dy >> 1, dx >> 1); [O][tap = oy*2+ox][phase = py*2+px][I], zeros elsewhere."""
-            O, I = wt.shape[:2]
-            out = torch.zeros(O, 2, 2, 2, 2, I, dtype=torch.float32, device=wt.device)     # [O][oy][ox][py][px][I]
-            w = wt.detach().float()
-            for dy in range(3):
-                for dx in range(3):
-                    out[:, dy >> 1, dx >> 1, dy & 1, dx & 1, :] = w[:, :, dy, dx]
-            return t16(out.reshape(O, -1))
+        conv16 = lambda wt: t16(pack_conv3x3(wt))      # noqa: E731
+        lin16 = lambda wt: t16(pack_linear(wt))        # noqa: E731
+        down16 = lambda wt: t16(pack_down2(wt))        # noqa: E731
 
         def resnet(r):
             s = _lib.VaeResnet()
@@ -314,7 +339,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
         e.attn_q_w16, e.attn_q_b = lin16(at.to_q.weight), f32(at.to_q.bias)
         e.attn_k_w16, e.attn_k_b = lin16(at.to_k.weight), f32(at.to_k.bias)
         e.attn_v_w16, e.attn_o_w16 = lin16(at.to_v.weight), lin16(at.to_out[0].weight)
-        e.attn_o_b = f32(at.to_out[0].bias.detach().float() + at.to_out[0].weight.detach().float() @ at.to_v.bias.detach().float())
+        e.attn_o_b = f32(fold_v_bias(at.to_out[0].weight, at.to_out[0].bias, at.to_v.bias))
         e.norm_out_g, e.norm_out_b = f32(enc.conv_norm_out.weight), f32(enc.conv_norm_out.bias)
         M = 2 * c.latent_channels
         wo = torch.zeros(32, *enc.conv_out.weight.shape[1:], dtype=torch.float32, device=dev)
@@ -373,21 +398,14 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             keep.append(t)
             return t.data_ptr()
 
-        def conv16(wt):  # OIHW -> [O][ky*3+kx][I]
-            t = wt.detach().permute(0, 2, 3, 1).reshape(wt.shape[0], -1).to(device=dev, dtype=od).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def lin16(wt):
-            t = wt.detach().reshape(wt.shape[0], -1).to(device=dev, dtype=od).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def conv16_t(wt, scale=1.0):  # Conv3d (3,1,1): [O][I][kt][1][1] -> [O][kt][I]
-            t = (wt.detach().float() * scale).reshape(wt.shape[0], wt.shape[1], 3).permute(0, 2, 1).reshape(wt.shape[0], -1)
+        def t16(t):
             t = t.to(device=dev, dtype=od).contiguous()
             keep.append(t)
             return t.data_ptr()
+
+        conv16 = lambda wt: t16(pack_conv3x3(wt))                           # noqa: E731
+        lin16 = lambda wt: t16(pack_linear(wt))                             # noqa: E731
+        conv16_t = lambda wt, scale=1.0: t16(pack_conv_t3(wt, scale))       # noqa: E731
 
         def resnet(blk):
             r = blk.spatial_res_block if self._temporal else blk
@@ -432,8 +450,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
         d.attn_k_w16, d.attn_k_b = lin16(at.to_k.weight), f32(at.to_k.bias)
         d.attn_v_w16 = lin16(at.to_v.weight)
         d.attn_o_w16 = lin16(at.to_out[0].weight)
-        # softmax rows sum to 1, so P (V + 1 b_v^T) W_o^T + b_o = P V W_o^T + (W_o b_v + b_o): fold the v bias
-        d.attn_o_b = f32(at.to_out[0].bias.detach().float() + at.to_out[0].weight.detach().float() @ at.to_v.bias.detach().float())
+        d.attn_o_b = f32(fold_v_bias(at.to_out[0].weight, at.to_out[0].bias, at.to_v.bias))
         for b, blk in enumerate(dec.up_blocks):
             for r in range(3):
                 d.up[b * 3 + r] = resnet(blk.resnets[r])

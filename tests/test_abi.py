@@ -71,6 +71,25 @@ def test_abi_version_and_error_text(lib):
     assert rc == -7 and "head_dim" in _lib.last_error()
 
 
+def test_vae_layer_argument_checks(lib):
+    """The single-layer VAE entry points validate shapes and pointers on the host, before any CUDA call."""
+    from latte_b200 import _lib
+    rc = lib.b200_vae_conv(None, None, None, None, None, None, 1, 16, 8, 96, 64, _lib.VAE_CONV3X3, _lib.FP16, None)
+    assert rc == -7 and "multiple of 64" in _lib.last_error()
+    rc = lib.b200_vae_conv(None, None, None, None, None, None, 1, 16, 8, 64, 128, _lib.VAE_CONV_T3, _lib.FP16, None)
+    assert rc == -7 and "C -> C" in _lib.last_error()
+    rc = lib.b200_vae_conv(None, None, None, None, None, None, 1, 16, 8, 64, 64, 9, _lib.FP16, None)
+    assert rc == -7 and "kind" in _lib.last_error()
+    assert lib.b200_vae_conv(None, None, None, None, None, None, 1, 16, 8, 64, 64, _lib.VAE_CONV_DOWN2, _lib.BF16, None) == -3
+    assert lib.b200_group_norm(None, None, None, None, None, 1, 128, 64, 16, 1e-6, 0, 5, None) == -2
+    assert lib.b200_group_norm(None, None, None, None, None, 1, 128, 64, 0, 1e-6, 0, 0, None) == -1
+    assert lib.b200_vae_mid_attention_workspace_bytes(1, 8, 16, 96, 32) == 0 and "multiple of 64" in _lib.last_error()
+    n, hw, C, G = 2, 128, 128, 32
+    ws = lib.b200_vae_mid_attention_workspace_bytes(n, 8, 16, C, G)
+    lower = 3 * n * hw * C * 2 + C * hw * 2 + hw * hw * (2 + 4) + hw * 4 + n * G * 8    # o, q, k, v^T, P, scores, ones, stats
+    assert lower <= ws < lower + 8 * 1024
+
+
 def test_workspace_size_formula(lib):
     from latte_b200 import _lib
     s = _lib.LatteShape(depth=28, hidden=1152, heads=16, mlp_hidden=4608, patch=2, in_channels=4, out_channels=8,
