@@ -145,6 +145,19 @@ __device__ __forceinline__ float gelu_tanh_grad(float x) {
   return fmaf(0.5f * x * sech2, k0 * fmaf(3.0f * k1, x2, 1.0f), fmaf(0.5f, t, 0.5f));
 }
 
+// the residual epilogue's increment gate * (acc + bias) (+ row_add), added to x by the caller; rounded step by step (no FMA
+// contraction) so that every path through the epilogue produces the same bits
+__device__ __forceinline__ float resid_delta(float acc, float b, float gt, float ra, bool has_ra) {
+  const float dv = __fmul_rn(gt, __fadd_rn(acc, b));
+  return has_ra ? __fadd_rn(dv, ra) : dv;
+}
+
+// column groups per batch of epilogue loads in the full-tile paths: all loads of a chunk are issued before its first use
+constexpr int kEpiChunk = 8;
+// ends a chunk: keeps the compiler (ptxas included: bar.warp.sync orders memory) from hoisting the next chunk's loads above
+// it, which would hold the loads of the whole tile in registers next to the accumulators and spill
+__device__ __forceinline__ void epi_chunk_fence() { __syncwarp(); }
+
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5 x (1 + tanh(u)),  u = sqrt(2/pi) (x + 0.044715 x^3).  ONE MUFU op per element (tanh.approx, rel. error 2^-11,
   // the same size as the 16-bit rounding of the result) instead of ex2 + rcp: the 16/clk/SM MUFU pipe is the fc1
@@ -160,6 +173,7 @@ template <int BN, int EPI, bool BF16>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
   using C = Cfg<BN, EPI>;
+  static_assert((BN / 8) % kEpiChunk == 0, "the epilogue chunks must tile the 8-column groups of a tile exactly");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
@@ -331,29 +345,56 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
           asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
         }
+        const float* bias = (p.bias && first_seg) ? p.bias : nullptr;
+        const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = r0 + 8 * h;
-          if (row >= p.M) continue;
-          const float* gate_row = p.gate + static_cast<long long>(row / p.rows_per_batch) * p.gate_bs;
-          const float* add_row = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((row / p.row_add_div) % p.row_add_period) * p.N : nullptr;
-          float* xrow = p.resid + static_cast<size_t>(row) * p.N;
-          const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+          // rows past M are skipped per lane (M need not be a multiple of 8, so one warp can hold both kinds); the row
+          // pointers are formed from a clamped row and never dereferenced for such a lane
+          const bool row_ok = row < p.M;
+          if (BN > 192 && !row_ok) continue;   // no chunked path (and no fence) at BN = 256: skip the row outright
+          const int prow = row_ok ? row : p.M - 1;
+          const float* gate_row = p.gate + static_cast<long long>(prow / p.rows_per_batch) * p.gate_bs;
+          const float* add_row = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((prow / p.row_add_div) % p.row_add_period) * p.N : nullptr;
+          float* xrow = p.resid + static_cast<size_t>(prow) * p.N;
+          if (BN <= 192 && live == BN / 8) {
+            // whole tile inside N: the x loads of a chunk of column groups (HBM / L2 round trips) are all in flight before
+            // the chunk's first store, instead of one dependent round trip per column group; gate, bias and row_add are
+            // L1-resident after the first warp's touch.  Not at BN = 256: beside its 128 accumulators the batch spills.
+            // Every lane of the warp reaches each chunk fence (a __syncwarp): rows past M only predicate the memory accesses.
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            if (j >= live) break;
-            const int col = n0 + 8 * j + 2 * cq;
-            float2 b2 = make_float2(0.f, 0.f);
-            if (p.bias && first_seg) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-            const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
-            float2 dv = make_float2(gt.x * (acc[4 * j + 2 * h] + b2.x), gt.y * (acc[4 * j + 2 * h + 1] + b2.y));
-            if (add_row) {
-              const float2 ra = __ldg(reinterpret_cast<const float2*>(add_row + col));
-              dv.x += ra.x; dv.y += ra.y;
+            for (int j0 = 0; j0 < BN / 8; j0 += kEpiChunk) {
+              float2 x[kEpiChunk];
+#pragma unroll
+              for (int j = 0; j < kEpiChunk; ++j)
+                if (row_ok) x[j] = *reinterpret_cast<const float2*>(xrow + n0 + 8 * (j0 + j) + 2 * cq);
+#pragma unroll
+              for (int j = 0; j < kEpiChunk; ++j) {
+                if (!row_ok) continue;
+                const int col = n0 + 8 * (j0 + j) + 2 * cq;
+                const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
+                const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
+                const float2 ra = add_row ? __ldg(reinterpret_cast<const float2*>(add_row + col)) : make_float2(0.f, 0.f);
+                x[j].x = __fadd_rn(x[j].x, resid_delta(acc[4 * (j0 + j) + 2 * h], b2.x, gt.x, ra.x, add_row != nullptr));
+                x[j].y = __fadd_rn(x[j].y, resid_delta(acc[4 * (j0 + j) + 2 * h + 1], b2.y, gt.y, ra.y, add_row != nullptr));
+                *reinterpret_cast<float2*>(xrow + col) = x[j];
+              }
+              epi_chunk_fence();
             }
-            float2 x = *reinterpret_cast<const float2*>(xrow + col);
-            x.x += dv.x; x.y += dv.y;
-            *reinterpret_cast<float2*>(xrow + col) = x;
+          } else if (row_ok) {
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              if (j >= live) break;
+              const int col = n0 + 8 * j + 2 * cq;
+              const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
+              const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
+              const float2 ra = add_row ? __ldg(reinterpret_cast<const float2*>(add_row + col)) : make_float2(0.f, 0.f);
+              float2 x = *reinterpret_cast<const float2*>(xrow + col);
+              x.x = __fadd_rn(x.x, resid_delta(acc[4 * j + 2 * h], b2.x, gt.x, ra.x, add_row != nullptr));
+              x.y = __fadd_rn(x.y, resid_delta(acc[4 * j + 2 * h + 1], b2.y, gt.y, ra.y, add_row != nullptr));
+              *reinterpret_cast<float2*>(xrow + col) = x;
+            }
           }
         }
         if (partial && kb1 < num_kb) {
@@ -362,41 +403,76 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (te == 0) flag_release(flag, static_cast<unsigned long long>(kb1));   // ... the next segment may add
         }
       } else {
+        bool done = false;
+        if constexpr (EPI == B200_EPI_BIAS || EPI == B200_EPI_BIAS_GELU) {
+          if (p.N - n0 >= BN) {
+            // whole tile inside N (bias / bias + GELU epilogues): a chunk's bias loads are issued together and shared by both
+            // row halves, instead of one dependent load before every store
+            const bool row_ok[2] = {r0 < p.M, r0 + 8 < p.M};
+            uint32_t* orow[2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          if (row >= p.M) continue;
-          uint32_t* orow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(row) * p.N);
-          const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+            for (int h = 0; h < 2; ++h)
+              orow[h] = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(r0 + 8 * h) * p.N);
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            if (j >= live) break;
-            const int col = n0 + 8 * j + 2 * cq;
-            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-            if (p.bias) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-              f0 += b.x; f1 += b.y;
+            for (int j0 = 0; j0 < BN / 8; j0 += kEpiChunk) {
+              float2 b[kEpiChunk];
+#pragma unroll
+              for (int j = 0; j < kEpiChunk; ++j)
+                b[j] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * (j0 + j) + 2 * cq)) : make_float2(0.f, 0.f);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                if (!row_ok[h]) continue;
+#pragma unroll
+                for (int j = 0; j < kEpiChunk; ++j) {
+                  const int col = n0 + 8 * (j0 + j) + 2 * cq;
+                  float f0 = acc[4 * (j0 + j) + 2 * h], f1 = acc[4 * (j0 + j) + 2 * h + 1];
+                  if (p.bias) { f0 += b[j].x; f1 += b[j].y; }
+                  if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+                  orow[h][col / 2] = pack2<BF16>(f0, f1);
+                }
+              }
+              epi_chunk_fence();
             }
-            if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
-            uint32_t val = pack2<BF16>(f0, f1);
-            const size_t off = (static_cast<size_t>(row) * p.N + col) / 2;
-            if constexpr (EPI == B200_EPI_BIAS_MUL16) {   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
-              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-              val = pack2<BF16>(a.x * r.x, a.y * r.y);
+            done = true;
+          }
+        }
+        if (!done) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            if (row >= p.M) continue;
+            uint32_t* orow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(row) * p.N);
+            const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              if (j >= live) break;
+              const int col = n0 + 8 * j + 2 * cq;
+              float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+              if (p.bias) {
+                const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                f0 += b.x; f1 += b.y;
+              }
+              if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+              uint32_t val = pack2<BF16>(f0, f1);
+              const size_t off = (static_cast<size_t>(row) * p.N + col) / 2;
+              if constexpr (EPI == B200_EPI_BIAS_MUL16) {   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
+                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+                val = pack2<BF16>(a.x * r.x, a.y * r.y);
+              }
+              if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) {   // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
+                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+                val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
+              }
+              if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) {   // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
+                const float2 a = unpack2<BF16>(val);
+                reinterpret_cast<uint32_t*>(p.out16b)[off] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
+              }
+              if constexpr (EPI == B200_EPI_BIAS_ADD16) {   // + shortcut, both already rounded to 16 bits like the reference
+                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
+                val = pack2<BF16>(a.x + r.x, a.y + r.y);
+              }
+              orow[col / 2] = val;
             }
-            if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) {   // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
-              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-              val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
-            }
-            if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) {   // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
-              const float2 a = unpack2<BF16>(val);
-              reinterpret_cast<uint32_t*>(p.out16b)[off] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
-            }
-            if constexpr (EPI == B200_EPI_BIAS_ADD16) {   // + shortcut, both already rounded to 16 bits like the reference
-              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-              val = pack2<BF16>(a.x + r.x, a.y + r.y);
-            }
-            orow[col / 2] = val;
           }
         }
       }

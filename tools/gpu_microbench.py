@@ -53,6 +53,11 @@ def gemm():
             for fl_on in (True, False):
                 best, mean = bench(fn, do_flush=fl_on)
                 print(f"gemm {name:4s} {M}x{N}x{K} bn{bn} {'cold' if fl_on else 'warm'}: best {best:7.1f} us mean {mean:7.1f} us -> {fl / best / 1e6:7.1f} TFLOP/s (best)", flush=True)
+            if mode == "resid":
+                # the same shape and tile width with the 16-bit bias epilogue instead: the difference to the line above is
+                # what the gated-residual epilogue (fp32 x read + written in place) costs over the mainloop
+                best, mean = bench(lambda: ops.linear(A, W, bias, block_n=bn), do_flush=True)
+                print(f"gemm {name:4s} {M}x{N}x{K} bn{bn} bias-epilogue cold: best {best:7.1f} us mean {mean:7.1f} us -> {fl / best / 1e6:7.1f} TFLOP/s (best)", flush=True)
 
 
 def attn():
