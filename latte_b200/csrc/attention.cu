@@ -7,10 +7,15 @@
 //   spatial  (temporal=0): a tile is 128 consecutive tokens of one frame; keys = the frame's N tokens, fetched in
 //            chunks of 128 rows.  3-D map {hd, 3H, T}; Q box {64|16, 1, 128}, K/V box {64|16, 1, 128}.
 //            N < 128: 128/N whole sequences are packed per tile with a block-diagonal mask (r/N == c/N).
-//   temporal (temporal=1): a tile is G = 128/F neighbouring tokens x all F frames, fetched with a 4-D map
-//            {hd, 3H, N, B*F} and box {64|16, 1, G, F} -> tile row r = f*G + g; the G sequences are masked
-//            block-diagonally (r % G == c % G).  Wasted tensor FLOPs (x G) are cheap; HBM traffic is minimal:
-//            every q/k/v element is read once, every output written once, no transpose pass.
+//   temporal (temporal=1): a tile is G = floor(128/F) neighbouring tokens x all F frames, fetched with a 4-D map
+//            {hd, 3H, N, B*F} and box {64|16, 1, G, F} -> tile row r = f*G + g < G*F <= 128; the G sequences are
+//            masked block-diagonally (c < G*F and r % G == c % G).  Wasted tensor FLOPs (x G) are cheap; HBM traffic
+//            is minimal: every q/k/v element is read once, every output written once, no transpose pass.
+//            When G does not divide N the last group of a sequence is partial: TMA zero-fills its missing tokens on
+//            load and clips them on store.  When G*F < 128, K/V rows [G*F, 128) are never loaded; the V rows are
+//            zeroed (P = 0 times stale NaN bits would be NaN), the K rows are removed by the mask select.
+//            F a power of two (G*F = 128) keeps the original xor mask (MODE_TEMPORAL); any other F in [1, 128] runs
+//            MODE_TEMPORAL_ANY.
 //   cross    (text conditioning, T5): queries of one sample against its <= 128 text keys, with an optional additive
 //            bias per key (mask) and per (head, query row, key) (T5's relative position bias).
 // head_dim 72 / 80 are not multiples of the K = 16 granule of the second product: the first 64 dims use 128B-swizzled
@@ -35,20 +40,20 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kChunk = 128;            // keys per K/V stage
 
-enum { MODE_FULL = 0, MODE_PACKED = 1, MODE_TEMPORAL = 2, MODE_CROSS = 3 };
+enum { MODE_FULL = 0, MODE_PACKED = 1, MODE_TEMPORAL = 2, MODE_CROSS = 3, MODE_TEMPORAL_ANY = 4 };
 
 struct AttnDev {
   int heads;
   int hd;
   int tokens;       // N
   int frames;       // F
-  int group;        // PACKED: N (tokens per sequence); TEMPORAL: G = 128 / F  (power of two)
-  int gshift;       // log2(group)
+  int group;        // PACKED: N (tokens per sequence); TEMPORAL: G = 128 / F  (power of two); TEMPORAL_ANY: floor(128 / F)
+  int gshift;       // log2(group)  (PACKED, TEMPORAL)
   int k_head0, v_head0;  // index of head 0 of K / V in the (hd, heads-like, rows) view of the K/V buffer
   int kv_rows_per_batch; // CROSS: rows of the K/V buffer per sample
   int q_rows_per_batch;  // CROSS: query rows per sample (F * N)
   int chunks;       // key chunks of 128 per tile: FULL N / 128, otherwise 1
-  int tiles_per_seq;  // FULL: N / 128; TEMPORAL: N / G
+  int tiles_per_seq;  // FULL: N / 128; TEMPORAL: N / G; TEMPORAL_ANY: ceil(N / G)
   float scale_log2; // score scale * log2(e)
   const float* key_bias;  // CROSS: additive bias on the scores, fp32 [batch][128] (natural-log units, e.g. 0 / -10000), or nullptr
   const float* pos_bias;  // CROSS: additive bias fp32 [heads][128][128] per (head, query row, key), or nullptr
@@ -88,10 +93,11 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   uint64_t* kv_full = bars + 1;    // [2]
   uint64_t* kv_empty = bars + 3;   // [2]
 
+  constexpr bool kTemporal = MODE == MODE_TEMPORAL || MODE == MODE_TEMPORAL_ANY;
   const int head = blockIdx.y, tile = blockIdx.x;
   // TMA coordinates of the tile: query rows (c2, c3), first key row kv2
   int c2, c3 = 0, kv2;
-  if constexpr (MODE == MODE_TEMPORAL) {
+  if constexpr (kTemporal) {
     c2 = (tile % p.tiles_per_seq) * p.group;        // first token of the group
     c3 = (tile / p.tiles_per_seq) * p.frames;       // first (b, f) image
     kv2 = c2;
@@ -106,13 +112,16 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     c2 = kv2 = tile * 128;
   }
   const int nchunks = MODE == MODE_FULL ? p.chunks : 1;
-  constexpr uint32_t kv_bytes = L::KV_BYTES;
+  // rows of a Q / K / V tile that TMA writes (out-of-bounds elements it zero-fills count towards the transaction bytes)
+  const int tile_rows = MODE == MODE_TEMPORAL_ANY ? p.group * p.frames : 128;
+  const uint32_t q_bytes = MODE == MODE_TEMPORAL_ANY ? tile_rows * (128u + (TAIL ? 32u : 0u)) : uint32_t(L::Q_BYTES);
+  const uint32_t kv_bytes = MODE == MODE_TEMPORAL_ANY ? 2u * q_bytes : uint32_t(L::KV_BYTES);
 
   auto load_kv = [&](int j) {
     uint8_t* st = smem + L::STAGE0 + (j & 1) * L::KV_BYTES;
     uint64_t* bar = kv_full + (j & 1);
     mbar_arrive_expect_tx(bar, kv_bytes);
-    if constexpr (MODE == MODE_TEMPORAL) {
+    if constexpr (kTemporal) {
       tma_load_4d(st + L::K_MAIN, &tmKV, bar, 0, p.k_head0 + head, kv2, c3);
       tma_load_4d(st + L::V_MAIN, &tmKV, bar, 0, p.v_head0 + head, kv2, c3);
       if constexpr (TAIL) {
@@ -141,12 +150,23 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     }
     fence_mbar_init();
   }
+  if constexpr (MODE == MODE_TEMPORAL_ANY) {
+    // V rows [tile_rows, 128) of the (only) stage are never loaded; zero them so that P = 0 multiplies zeros, not stale
+    // bits.  Whole rows: a row stays a row under both the 128B and the 32B swizzle.  TMA writes rows [0, tile_rows) only.
+    uint8_t* st = smem + L::STAGE0;
+    const int main_chunks = (128 - tile_rows) * 8, n = main_chunks + (TAIL ? (128 - tile_rows) * 2 : 0);
+    for (int i = threadIdx.x; i < n; i += kThreads) {
+      uint8_t* dst = i < main_chunks ? st + L::V_MAIN + tile_rows * 128 + i * 16 : st + L::V_TAIL + tile_rows * 32 + (i - main_chunks) * 16;
+      *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    fence_proxy_async_smem();     // the zeros are read by wgmma (async proxy) after the barrier below
+  }
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();   // qkv (written by the preceding GEMM) is visible from here
   if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(q_full, L::Q_BYTES);
-    if constexpr (MODE == MODE_TEMPORAL) {
+    mbar_arrive_expect_tx(q_full, q_bytes);
+    if constexpr (kTemporal) {
       tma_load_4d(smem + L::Q_MAIN, &tmQ, q_full, 0, head, c2, c3);
       if constexpr (TAIL) tma_load_4d(smem + L::Q_TAIL, &tmQt, q_full, 64, head, c2, c3);
     } else {
@@ -163,6 +183,26 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   const int g = lane >> 2, cq = lane & 3;
   const int rA = wg * 64 + (te >> 5) * 16 + g;    // tile rows of this thread: rA and rA + 8
   const int rows[2] = {rA, rA + 8};
+  // TEMPORAL_ANY: bit 2*j8 + e of kmask[h] says whether key column c = 8*j8 + 2*cq + e is valid for row rows[h]
+  // (c < G*F and c % G == rows[h] % G).  Residues are stepped by 8 % G per j8 instead of divided per score.
+  uint32_t kmask[2] = {0u, 0u};
+  if constexpr (MODE == MODE_TEMPORAL_ANY) {
+    const int G = p.group, step = 8 % G;
+    const int rres[2] = {rows[0] % G, rows[1] % G};
+    int cres[2] = {(2 * cq) % G, (2 * cq + 1) % G};
+#pragma unroll
+    for (int j8 = 0; j8 < 16; ++j8) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const bool in_tile = 8 * j8 + 2 * cq + e < tile_rows;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          kmask[h] |= (in_tile && cres[e] == rres[h]) ? 1u << (2 * j8 + e) : 0u;
+        cres[e] += step;
+        cres[e] -= cres[e] >= G ? G : 0;
+      }
+    }
+  }
 
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   float o[32], ot[8];
@@ -219,6 +259,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
           bool valid = true;
           if constexpr (MODE == MODE_PACKED) valid = (r >> p.gshift) == (c >> p.gshift);
           if constexpr (MODE == MODE_TEMPORAL) valid = ((r ^ c) & ((1 << p.gshift) - 1)) == 0;
+          if constexpr (MODE == MODE_TEMPORAL_ANY) valid = (kmask[h] >> (2 * j8 + e)) & 1u;
           if constexpr (MODE == MODE_CROSS) {
             valid = c < p.kv_valid;
             if (kbias) x = fmaf(__ldg(kbias + c), kLog2e, x);
@@ -316,7 +357,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   fence_proxy_async_smem();       // the staging tile is read by the TMA engine
   asm volatile("bar.sync 1, 256;" ::: "memory");
   if (threadIdx.x == 0) {
-    if constexpr (MODE == MODE_TEMPORAL) tma_store_4d(&tmO, stage_out, 0, head, c2, c3);
+    if constexpr (kTemporal) tma_store_4d(&tmO, stage_out, 0, head, c2, c3);
     else tma_store_3d(&tmO, stage_out, 0, head, c2);
     tma_store_commit();
     tma_store_wait_all<0>();
@@ -338,6 +379,7 @@ int launch_tail(int mode, const CUtensorMap* m, const AttnDev& p, dim3 grid, cud
     case MODE_FULL: return launch_mode<BF16, TAIL, MODE_FULL>(m, p, grid, s);
     case MODE_PACKED: return launch_mode<BF16, TAIL, MODE_PACKED>(m, p, grid, s);
     case MODE_CROSS: return launch_mode<BF16, TAIL, MODE_CROSS>(m, p, grid, s);
+    case MODE_TEMPORAL_ANY: return launch_mode<BF16, TAIL, MODE_TEMPORAL_ANY>(m, p, grid, s);
     default: return launch_mode<BF16, TAIL, MODE_TEMPORAL>(m, p, grid, s);
   }
 }
@@ -419,14 +461,13 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
     }
   } else {
     const int F = a.frames;
-    B200_REQUIRE(F >= 4 && F <= 128 && 128 % F == 0, B200_ERR_UNSUPPORTED,
-                 "attention: temporal length %d unsupported (power of two in [4,128])", F);
+    B200_REQUIRE(F >= 1 && F <= 128, B200_ERR_UNSUPPORTED, "attention: temporal length %d unsupported (1..128)", F);
     const int G = 128 / F;
-    B200_REQUIRE(a.tokens % G == 0, B200_ERR_UNSUPPORTED, "attention: tokens %d must be a multiple of %d", a.tokens, G);
-    mode = MODE_TEMPORAL;
+    // G * F == 128 exactly when F is a power of two: the full tile keeps the xor mask and compile-time byte counts
+    mode = G * F == 128 ? MODE_TEMPORAL : MODE_TEMPORAL_ANY;
     p.group = G;
     p.gshift = ilog2(G);
-    p.tiles_per_seq = a.tokens / G;
+    p.tiles_per_seq = (a.tokens + G - 1) / G;
     grid = dim3(static_cast<unsigned>(a.batch * p.tiles_per_seq), H);
     const uint64_t dims[4] = {static_cast<uint64_t>(hd), static_cast<uint64_t>(3 * H), static_cast<uint64_t>(a.tokens),
                               static_cast<uint64_t>(a.batch) * F};
