@@ -102,7 +102,8 @@ struct GemmArgs {
   int w_const;          // 1: W is a constant weight matrix (never written during the step); a scheduling hint the
                         // current kernel does not need (every operand is fetched after the grid dependency resolves)
   int mn_major;         // bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (N % 128 == 0).  3 = wgrad (dW[M, N] += dY[K, M]^T X[K, N]),
-                        // 2 = dgrad (dX[M, N] = dY[M, K] W[K, N] with the weight in its nn.Linear [out, in] layout)
+                        // 2 = dgrad (dX[M, N] = dY[M, K] W[K, N] with the weight in its nn.Linear [out, in] layout);
+                        // 1 is rejected (no caller transposes A alone)
   unsigned long long* sk_flags;  // B200_GEMM_SK_FLAGS zeroed u64 (caller's workspace) or nullptr: enables ordered stream-K
   const void* add16;    // EPI_BIAS_ADD16: [M, N] 16-bit tensor added to the result (resnet shortcut); EPI_BIAS_MUL16 / EPI_MUL_GELUGRAD16: the factor
   void* out16b;         // EPI_BIAS_GELU_BOTH: [M, N] 16-bit second output = gelu_tanh(out16)

@@ -10,12 +10,14 @@
 // Hopper structure: CTAs run as PAIRS (cluster of 2).  A pair owns a 256 x BN pair-tile: each CTA multiplies its own 128 A
 // rows, and each fetches only HALF of the W tile and multicasts it into both CTAs' shared memory (TMA .multicast::cluster),
 // so every W byte crosses L2 -> SM once per pair.
-//   thread 0        also the TMA producer: A tile 128x64 and the W half (BN/2)x64 (128B-swizzled) per pipeline stage;
-//                   a stage is full when this CTA's A bytes and BOTH W halves have landed on its "full" barrier.  (A
-//                   separate producer warp would cap every thread at 168 registers; the 64 x 256 accumulator needs 128.)
-//   warpgroups 0-1  wgmma (64 x BN x 16, fp32 accumulators in registers), one 64-row half of the tile each, then the
-//                   epilogue straight from the accumulator registers; a stage is released with one arrival per warpgroup on
-//                   the "empty" barriers of BOTH CTAs (the peer's next multicast writes into it)
+// 384 threads, warp-specialized; setmaxnreg moves registers from the producer (40 per thread) to the consumers (232):
+//   warpgroup 0     the TMA producer, one thread: A tile 128x64 and the W half (BN/2)x64 (128B-swizzled) per pipeline
+//                   stage; a stage is full when this CTA's A bytes and BOTH W halves have landed on its "full" barrier.
+//                   It waits only on "empty" and keeps every stage in flight, through the consumers' epilogues.
+//   warpgroups 1-2  the consumers: wgmma (64 x BN x 16, fp32 accumulators in registers), one 64-row half of the tile each,
+//                   then the epilogue straight from the accumulator registers; they wait only on "full", and a stage is
+//                   released with one arrival per warpgroup on the "empty" barriers of BOTH CTAs (the peer's next
+//                   multicast writes into it)
 //
 // Residual epilogue: every element of x is owned by one thread and updated in place (x += gate * (acc + bias) (+ row_add)),
 // once per GEMM -- or, for the stream-K tiles of the last waves, once per K segment in k order (TileSched below).
@@ -32,7 +34,11 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 x 16-bit = one 128-byte swizzle row
-constexpr int kThreads = 256;   // warpgroups 0-1 MMA + epilogue; thread 0 also issues the TMA loads
+constexpr int kThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1-2: MMA + epilogue
+// per-thread registers after setmaxnreg.  The kernel is compiled for 65536 / 384 -> 168; the producer's release pays for
+// the consumers' raise exactly: 128 * (168 - 40) = 256 * (232 - 168), and (40 + 2 * 232) * 128 = 64,512 fit the SM's 65,536.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 
 template <int BN, int EPI>
 struct Cfg {
@@ -65,9 +71,6 @@ struct GemmDev {
   // implicit-GEMM convolution: see GemmArgs
   int conv_taps, conv_cblk, conv_h, conv_w, conv_bw, conv_bh;
   int conv_dx[9], conv_dy[9], conv_dz[9];
-  int mn_major; // bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (the contraction dimension is the ROW index): such an
-                // operand is fetched as 64-wide MN blocks x 64 k-rows and multiplied through an MN-major wgmma descriptor.
-                // wgrad sets both (dW = dY^T X), dgrad only bit 1 (dX = dY W with W in its [out, in] layout).
   float* resid; // EPI_GATE_RESIDUAL: [M, N] fp32 residual stream, updated in place
   int streamk;  // residual epilogue only: split the last partial wave of tiles along K across all pairs (see TileSched)
   // stream-K ordering flags (caller's workspace), one per (streamed tile, CTA rank, epilogue warpgroup): "k-blocks of the
@@ -169,10 +172,17 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return fmaf(hx, t, hx);
 }
 
-template <int BN, int EPI, bool BF16>
+// MN: operand layout.  Bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (the contraction dimension is the ROW index):
+// such an operand is fetched as 64-wide MN blocks x 64 k-rows and multiplied through an MN-major wgmma descriptor.
+// wgrad uses 3 (dW = dY^T X), dgrad 2 (dX = dY W with W in its [out, in] layout), everything else 0.  A compile-time
+// layout keeps one straight-line wgmma sequence per k-block: a run-time choice between four makes ptxas join them with
+// an injected empty wgmma group, which turns wgmma_wait<1> into a full drain.
+template <int BN, int EPI, bool BF16, int MN>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
   using C = Cfg<BN, EPI>;
+  constexpr int TA = MN & 1, TB = MN >> 1;
+  static_assert(MN == 0 || MN == 2 || MN == 3, "operand layouts: 0 forward, 2 dgrad, 3 wgrad");
   static_assert((BN / 8) % kEpiChunk == 0, "the epilogue chunks must tile the 8-column groups of a tile exactly");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -188,7 +198,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full[i], 1);    // this CTA's expect_tx arrival; the bytes of both W halves and of A complete it
-      mbar_init(&empty[i], 4);   // one arrival per MMA warpgroup of BOTH CTAs (each W half lands in both)
+      mbar_init(&empty[i], 4);   // one arrival per consumer warpgroup of BOTH CTAs (each W half lands in both)
     }
     fence_mbar_init();
   }
@@ -205,67 +215,65 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int num_kb = p.K / BK;
   const bool streamk = C::RESID && p.streamk != 0;
 
-  // ------------------------------------------------------------------ TMA producer (thread 0, between its own MMAs)
-  // Load q of this CTA's k-block sequence goes to slot q % STAGES; it is issued once the slot's previous contents (load
-  // q - STAGES) have been released by both warpgroups of both CTAs.  Loads run up to STAGES - 1 k-blocks ahead of the MMAs,
-  // across tile boundaries, so the next tile's operands stream in while the epilogue runs.
-  TileSched lsched(my_pair, num_pairs, num_tiles, num_kb, streamk);
-  int l_tile = 0, l_kb = 0, l_kb1 = 0;
-  long long issued = 0;
-  bool l_more = true;
-  auto issue_one = [&]() {
-    if (l_kb == l_kb1) {
-      if (!(l_more = lsched.next(l_tile, l_kb, l_kb1))) return;
-    }
-    const int stage = static_cast<int>(issued % C::STAGES);
-    const uint32_t phase = static_cast<uint32_t>(issued / C::STAGES) & 1u;
-    const int m_blk = 2 * (l_tile / p.num_n) + static_cast<int>(rank), n_blk = l_tile % p.num_n;
-    const int w_row0 = n_blk * BN + static_cast<int>(rank) * (BN / 2);   // this CTA fetches half of the W tile for both
-    const int kb = l_kb++;
-    ++issued;
-    mbar_wait(&empty[stage], phase ^ 1);        // both CTAs' warpgroups are done with the slot
-    mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
-    uint8_t* sa = smem + stage * C::STAGE_BYTES;
-    if (p.conv_taps > 0) {
-      // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
-      // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
-      const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
-      const int pix0 = m_blk * BM;
-      const int hw = p.conv_h * p.conv_w;
-      const int img = pix0 / hw, rem = pix0 % hw;
-      tma_load_4d(sa, &tmA, &full[stage], cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap],
-                  img + p.conv_dz[tap]);
-    } else if (p.mn_major & 1) {
-      // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
-      // MN-major SW128 block; blocks past the live rows are zero-filled by TMA and still count their bytes
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer: warpgroup 0, one thread
+    // Load q of this CTA's k-block sequence goes to slot q % STAGES; it is issued as soon as the slot's previous contents
+    // (load q - STAGES) have been released by both consumer warpgroups of both CTAs, so all STAGES slots stay in flight,
+    // across tile boundaries and through the consumers' epilogues.  The producer waits on nothing but `empty`.
+    setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) {
+      pdl_wait();                             // operands: visible from here
+      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
+      int stage = 0;
+      uint32_t phase = 0;
+      int tile, kb0, kb1;
+      while (sched.next(tile, kb0, kb1)) {
+        const int m_blk = 2 * (tile / p.num_n) + static_cast<int>(rank), n_blk = tile % p.num_n;
+        const int w_row0 = n_blk * BN + static_cast<int>(rank) * (BN / 2);   // this CTA fetches half of the W tile for both
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);  // both CTAs' consumer warpgroups are done with the slot
+          mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
+          uint8_t* sa = smem + stage * C::STAGE_BYTES;
+          if (MN == 0 && p.conv_taps > 0) {
+            // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
+            // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
+            const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
+            const int pix0 = m_blk * BM;
+            const int hw = p.conv_h * p.conv_w;
+            const int img = pix0 / hw, rem = pix0 % hw;
+            tma_load_4d(sa, &tmA, &full[stage], cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap],
+                        img + p.conv_dz[tap]);
+          } else if constexpr (TA) {
+            // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
+            // MN-major SW128 block; blocks past the live rows are zero-filled by TMA and still count their bytes
 #pragma unroll
-      for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, &full[stage], m_blk * BM + j * 64, kb * BK);
-    } else {
-      tma_load_2d(sa, &tmA, &full[stage], kb * BK, m_blk * BM);
-    }
-    if (p.mn_major & 2) {
-      constexpr int per_cta = BN / 128;          // 64-column blocks of W this CTA fetches
+            for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, &full[stage], m_blk * BM + j * 64, kb * BK);
+          } else {
+            tma_load_2d(sa, &tmA, &full[stage], kb * BK, m_blk * BM);
+          }
+          if constexpr (TB) {
+            constexpr int per_cta = BN / 128;    // 64-column blocks of W this CTA fetches
 #pragma unroll
-      for (int j = 0; j < per_cta; ++j)
-        tma_load_2d_mcast(sa + C::A_BYTES + (rank * per_cta + j) * 8192, &tmB, &full[stage], w_row0 + j * 64, kb * BK, 0x3);
-    } else {
-      tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK, w_row0, 0x3);
+            for (int j = 0; j < per_cta; ++j)
+              tma_load_2d_mcast(sa + C::A_BYTES + (rank * per_cta + j) * 8192, &tmB, &full[stage], w_row0 + j * 64, kb * BK, 0x3);
+          } else {
+            tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK, w_row0, 0x3);
+          }
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
     }
-  };
-
-  pdl_wait();                                 // operands, bias / gate / shortcut / residual stream: visible from here
-  const bool producer = threadIdx.x == 0;
-  if (producer)
-    for (int i = 0; i < C::STAGES - 1 && l_more; ++i) issue_one();
-  {
-    // ------------------------------------------------------------------ MMA + epilogue warpgroups 0, 1 (64 rows each)
-    const int wg = warp >> 2;
+    __syncwarp();                             // warp 0 reconverges before the cluster barrier
+  } else {
+    // ------------------------------------------------------------------ MMA + epilogue: warpgroups 1, 2 (64 rows each)
+    setmaxnreg_inc<kConsumerRegs>();
+    pdl_wait();                               // bias / gate / shortcut / residual stream: visible from here
+    const int wg = (warp >> 2) - 1;           // which 64-row half of the tile
     const int te = threadIdx.x & 127;
     const int w4 = te >> 5, g = lane >> 2, cq = lane & 3;
     const uint32_t empty_peer = mapa_u32(&empty[0], rank ^ 1u);
     int stage = 0;
     uint32_t phase = 0;
-    long long consumed = 0;
     float acc[BN / 2];
     TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
     int tile, kb0, kb1;
@@ -278,36 +286,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         wgmma_fence();
         // K-major: 8-row groups 1024 B apart, a k-step of 16 elements = 32 B inside the swizzle row.  MN-major: 64-wide
         // blocks 8192 B apart (leading offset), 8-k-row groups 1024 B apart, a k-step of 16 k-rows = 2048 B.
-        switch (p.mn_major) {
-          case 0: {
-            const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
+        const uint64_t da = gmma_desc(sa + wg * 8192, TA ? 8192 : 16, 1024, GMMA_LAYOUT_SW128);
+        const uint64_t db = gmma_desc(sb, TB ? 8192 : 16, 1024, GMMA_LAYOUT_SW128);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              WgmmaSS<BN, 0, 0, BF16>::mma(acc, gmma_desc_advance(da, k * 32), gmma_desc_advance(db, k * 32), (kb != kb0 || k) ? 1u : 0u);
-            break;
-          }
-          case 2: {
-            const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 8192, 1024, GMMA_LAYOUT_SW128);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              WgmmaSS<BN, 0, 1, BF16>::mma(acc, gmma_desc_advance(da, k * 32), gmma_desc_advance(db, k * 2048), (kb != kb0 || k) ? 1u : 0u);
-            break;
-          }
-          case 1: {
-            const uint64_t da = gmma_desc(sa + wg * 8192, 8192, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              WgmmaSS<BN, 1, 0, BF16>::mma(acc, gmma_desc_advance(da, k * 2048), gmma_desc_advance(db, k * 32), (kb != kb0 || k) ? 1u : 0u);
-            break;
-          }
-          default: {
-            const uint64_t da = gmma_desc(sa + wg * 8192, 8192, 1024, GMMA_LAYOUT_SW128), db = gmma_desc(sb, 8192, 1024, GMMA_LAYOUT_SW128);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              WgmmaSS<BN, 1, 1, BF16>::mma(acc, gmma_desc_advance(da, k * 2048), gmma_desc_advance(db, k * 2048), (kb != kb0 || k) ? 1u : 0u);
-            break;
-          }
-        }
+        for (int k = 0; k < BK / 16; ++k)
+          WgmmaSS<BN, TA, TB, BF16>::mma(acc, gmma_desc_advance(da, k * (TA ? 2048 : 32)),
+                                         gmma_desc_advance(db, k * (TB ? 2048 : 32)), (kb != kb0 || k) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();                      // the previous k-block's MMAs have read their slot: release it in both CTAs
         if (prev >= 0 && te == 0) {
@@ -316,9 +300,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        ++consumed;
-        if (producer)
-          while (l_more && issued < consumed + C::STAGES - 1) issue_one();
       }
       wgmma_wait<0>();
       reg_fence(acc);
@@ -482,33 +463,44 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   cluster_sync_all();   // the peer may still multicast into our smem / arrive on our barriers until it is done too
 }
 
-template <int BN, int EPI, bool BF16>
+template <int BN, int EPI, bool BF16, int MN>
 int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t stream) {
   using C = Cfg<BN, EPI>;
-  auto kern = gemm_kernel<BN, EPI, BF16>;
+  auto kern = gemm_kernel<BN, EPI, BF16, MN>;
   B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
   B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tmA, tmB, p));
   return B200_OK;
 }
 
+// Only the (epilogue, operand layout) pairs that callers launch are instantiated: every epilogue with K-major operands,
+// dgrad's bias / GELU-gradient with W stored [K, N], and wgrad's unit-gate accumulation with both operands transposed
+// (transposed operands take 128- or 256-wide tiles only).
 template <int BN, bool BF16>
-int launch_epi(int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
-  switch (epi) {
-    case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16>(tmA, tmB, p, grid, s);
-    case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16>(tmA, tmB, p, grid, s);
+int launch_epi(int epi, int mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
+  if (mn == 0) {
+    switch (epi) {
+      case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 0>(tmA, tmB, p, grid, s);
+    }
   }
-  set_error("gemm: unknown epilogue %d", epi);
+  if constexpr (BN != 192) {
+    if (mn == 2 && epi == B200_EPI_BIAS) return launch_one<BN, B200_EPI_BIAS, BF16, 2>(tmA, tmB, p, grid, s);
+    if (mn == 2 && epi == B200_EPI_MUL_GELUGRAD16) return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 2>(tmA, tmB, p, grid, s);
+    if (mn == 3 && epi == B200_EPI_GATE_RESIDUAL) return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 3>(tmA, tmB, p, grid, s);
+  }
+  set_error("gemm: epilogue %d with operand layout %d and block_n %d is not built", epi, mn, BN);
   return B200_ERR_UNSUPPORTED;
 }
 
 template <int BN>
-int launch_bn(int bf16, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
-  return bf16 ? launch_epi<BN, true>(epi, tmA, tmB, p, grid, s) : launch_epi<BN, false>(epi, tmA, tmB, p, grid, s);
+int launch_bn(int bf16, int epi, int mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid,
+              cudaStream_t s) {
+  return bf16 ? launch_epi<BN, true>(epi, mn, tmA, tmB, p, grid, s) : launch_epi<BN, false>(epi, mn, tmA, tmB, p, grid, s);
 }
 
 constexpr int kStreamKMinKb = 32;          // K / 64 below which the split costs more than the idle tail it removes
@@ -625,9 +617,10 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
                "gemm: block_n must be 128, 192 or 256 (got %d)", a.block_n);
   int block_n = a.block_n;
   if (a.mn_major) {
-    B200_REQUIRE(a.mn_major >= 1 && a.mn_major <= 3 && a.conv_taps == 0 && (!(a.mn_major & 1) || a.M % 8 == 0) &&
+    B200_REQUIRE((a.mn_major == 2 || a.mn_major == 3) && a.conv_taps == 0 && (!(a.mn_major & 1) || a.M % 8 == 0) &&
                      (!(a.mn_major & 2) || a.N % 128 == 0) && (a.block_n == 0 || a.block_n == 128 || a.block_n == 256),
-                 B200_ERR_UNSUPPORTED, "gemm (transposed operands): M %% 8 == 0, N %% 128 == 0, block_n 128 or 256 (M=%d N=%d)", a.M, a.N);
+                 B200_ERR_UNSUPPORTED, "gemm (transposed operands): mn_major 2 or 3, M %% 8 == 0, N %% 128 == 0, block_n 128 or 256 (M=%d N=%d)",
+                 a.M, a.N);
     if (block_n == 0) {
       block_n = pick_block_n(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, sms);
       if (block_n == 192) block_n = (a.N % 256 == 0 || a.N > 1024) ? 256 : 128;     // W chunks are 64 wide per CTA: 128 or 256 only
@@ -699,7 +692,6 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   p.conv_h = a.conv_h; p.conv_w = a.conv_w; p.conv_bw = conv_bw; p.conv_bh = conv_bh;
   for (int i = 0; i < 9; ++i) { p.conv_dx[i] = a.conv_dx[i]; p.conv_dy[i] = a.conv_dy[i]; p.conv_dz[i] = a.conv_dz[i]; }
   p.resid = a.resid;
-  p.mn_major = a.mn_major;
   const int pair_tiles = plan.pair_tiles;
   const int grid = 2 * plan.pairs;
   {
@@ -713,9 +705,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     p.sk_flags = p.streamk ? a.sk_flags : nullptr;
   }
   switch (bn) {
-    case 128: return launch_bn<128>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
-    case 192: return launch_bn<192>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
-    default: return launch_bn<256>(a.bf16, a.epilogue, tmA, tmB, p, grid, stream);
+    case 128: return launch_bn<128>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
+    case 192: return launch_bn<192>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
+    default: return launch_bn<256>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
   }
 }
 

@@ -104,6 +104,15 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   }
 }
 
+// ----------------------------------------------------------------------------- per-warpgroup register budget
+// A warp-specialized kernel compiled for R registers per thread moves registers from its producer warpgroup (dec) to its
+// consumer warpgroups (inc) through the CTA's pool; inc blocks until the pool holds enough, so the budgets must balance
+// against R.  Every warp of the warpgroup executes the same instruction; N is a multiple of 8 in [24, 256].
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ----------------------------------------------------------------------------- proxies / fences
 __device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> visible to async proxy (wgmma/TMA)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
