@@ -6,7 +6,8 @@
 //   gate_bwd                       dm = dx * gate[b]; dgate[b] = sum_rows dx * m; dbias = sum_rows dm   (latte.py:179-180)
 //   ln_modulate_bwd                d/dx of LN(x)(1+scale)+shift accumulated into dx; dshift, dscale per sample (latte.py:28-29)
 //   attn_bwd_dq / attn_bwd_dkv     softmax(QK^T hd^-1/2)V backward on mma.sync tensor cores, scores recomputed (latte.py:48-77)
-//   attn_bwd_temporal              same for the F <= 16 frame sequences (CUDA cores, HBM-bound)
+//                                  (also the temporal sequences of 17..128 frames: strided rows, partial last block masked)
+//   attn_bwd_temporal(_mma)        same for the F <= 16 frame sequences (one 16-row tile per (b, n, head))
 //   ada_outer / ada_dsc            gradients of the stacked adaLN_modulation Linear on B rows  (latte.py:160-163,192-195)
 // All are HBM-bound passes (one read, one write, fp32 math) except the attention backward (tensor cores, ~2 % of the FLOPs).
 #include "common.h"
@@ -622,15 +623,26 @@ __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void cp_async4(void* dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
 
-// asynchronous copy of a [64 x HD] block (rows row0.., columns col0..col0+HD) of a row-major 16-bit matrix into a shared tile
-template <int HD>
-__device__ __forceinline__ void load_tile64(uint16_t* s, const uint16_t* __restrict__ g, size_t row0, int ld, int col0) {
+// asynchronous copy of a [64 x HD] block (rows row0.., columns col0..col0+HD) of a row-major 16-bit matrix into a shared tile.
+// STRIDED (temporal sequences): tile row r is matrix row row0 + r * rs for r < nvalid; rows r >= nvalid are past the end of the
+// sequence and are written with zeros, never left stale (a stale NaN would survive P = 0 in the MMAs).
+template <int HD, bool STRIDED = false>
+__device__ __forceinline__ void load_tile64(uint16_t* s, const uint16_t* __restrict__ g, size_t row0, int ld, int col0, int rs = 1,
+                                            int nvalid = 64) {
   constexpr int CH = HD / 8;          // 16-byte chunks per row
   constexpr int HDP = AB<HD>::HDP;
   for (int i = threadIdx.x; i < 64 * CH; i += blockDim.x) {
     const int r = i / CH, c = i % CH;
-    cp_async16(s + r * HDP + c * 8, g + (row0 + r) * ld + col0 + c * 8);
+    if constexpr (STRIDED) {
+      if (r < nvalid) cp_async16(s + r * HDP + c * 8, g + (row0 + static_cast<size_t>(r) * rs) * ld + col0 + c * 8);
+      else *reinterpret_cast<uint4*>(s + r * HDP + c * 8) = make_uint4(0, 0, 0, 0);
+    } else {
+      cp_async16(s + r * HDP + c * 8, g + (row0 + r) * ld + col0 + c * 8);
+    }
   }
 }
 // zero the pad columns [HD, KP) of `ntiles` consecutive tiles once (the copies above never touch them)
@@ -699,28 +711,51 @@ __device__ __forceinline__ void acc_to_afrag(uint32_t (&p)[4][4], const float (&
   }
 }
 
-// write a warp's [16 x HD] fp32 accumulator as 16-bit rows of the output (row pitch ld)
-template <bool BF16, int HD>
+// write a warp's [16 x HD] fp32 accumulator as 16-bit rows of the output (row pitch ld; STRIDED: tile row r is row row0 + r * rs)
+template <bool BF16, int HD, bool STRIDED = false>
 __device__ __forceinline__ void store_rows(uint16_t* __restrict__ g, size_t row0, int ld, int col0, const float (&acc)[AB<HD>::NT][4],
-                                           int r_in_tile, int nvalid) {
+                                           int r_in_tile, int nvalid, int rs = 1) {
   const int lane = threadIdx.x & 31;
   const int r = r_in_tile + (lane >> 2);
+  if constexpr (STRIDED) {
+    const size_t ra = row0 + static_cast<size_t>(r) * rs, rb = ra + static_cast<size_t>(8) * rs;
 #pragma unroll
-  for (int n = 0; n < AB<HD>::NT; ++n) {
-    const int c = col0 + n * 8 + (lane & 3) * 2;
-    if (r < nvalid) *reinterpret_cast<uint32_t*>(g + (row0 + r) * ld + c) = pack2<BF16>(acc[n][0], acc[n][1]);
-    if (r + 8 < nvalid) *reinterpret_cast<uint32_t*>(g + (row0 + r + 8) * ld + c) = pack2<BF16>(acc[n][2], acc[n][3]);
+    for (int n = 0; n < AB<HD>::NT; ++n) {
+      const int c = col0 + n * 8 + (lane & 3) * 2;
+      if (r < nvalid) *reinterpret_cast<uint32_t*>(g + ra * ld + c) = pack2<BF16>(acc[n][0], acc[n][1]);
+      if (r + 8 < nvalid) *reinterpret_cast<uint32_t*>(g + rb * ld + c) = pack2<BF16>(acc[n][2], acc[n][3]);
+    }
+  } else {
+#pragma unroll
+    for (int n = 0; n < AB<HD>::NT; ++n) {
+      const int c = col0 + n * 8 + (lane & 3) * 2;
+      if (r < nvalid) *reinterpret_cast<uint32_t*>(g + (row0 + r) * ld + c) = pack2<BF16>(acc[n][0], acc[n][1]);
+      if (r + 8 < nvalid) *reinterpret_cast<uint32_t*>(g + (row0 + r + 8) * ld + c) = pack2<BF16>(acc[n][2], acc[n][3]);
+    }
   }
+}
+
+// -inf for the key columns >= lim of a warp's [16 x 64] score block (the last, partial key block of a temporal sequence).
+// The column of accumulator element (n, e) is n * 8 + (lane & 3) * 2 + (e & 1): one compare per score, no division.
+__device__ __forceinline__ void mask_keys(float (&acc)[8][4], int lim) {
+  const int c0 = (threadIdx.x & 3) * 2;
+#pragma unroll
+  for (int n = 0; n < 8; ++n)
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (n * 8 + c0 + (e & 1) >= lim) acc[n][e] = -INFINITY;
 }
 
 // Kernel A: one CTA = 64 query rows of one (sequence, head).  Pass 1 recomputes the row statistics (log-sum-exp in log2
 // units) and delta = sum_d dO.O, stores both for kernel B; pass 2 recomputes P, forms dS = P (dP - delta) * scale and
 // accumulates dQ = dS K.  K / V blocks are double-buffered with cp.async so the next block streams in under the MMAs.
-template <bool BF16, int HD>
+// STRIDED: a sequence is the S frames of one (b, n) of the (b, f, n) row layout (row stride rs = tokens per frame, any S);
+// rows of the last block at or beyond S are zero-filled, their keys masked to -inf, and nothing of them is stored.
+template <bool BF16, int HD, bool STRIDED = false>
 __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ o,
                                                           const uint16_t* __restrict__ d_o, uint16_t* __restrict__ dqkv,
                                                           float* __restrict__ lse, float* __restrict__ delta, int S, int heads,
-                                                          float scale_log2) {
+                                                          float scale_log2, int rs) {
   using G = AB<HD>;
   extern __shared__ __align__(16) uint16_t sm[];
   uint16_t* sQ = sm;
@@ -730,14 +765,18 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
   const int qb = blockIdx.x, h = blockIdx.y, seq = blockIdx.z;
   const int D = heads * HD, ld = 3 * D;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const size_t seq_row0 = static_cast<size_t>(seq) * S;
+  const size_t seq_row0 = STRIDED ? static_cast<size_t>(seq / rs) * S * rs + seq % rs : static_cast<size_t>(seq) * S;
   const int q0 = qb * 64;
-  const int nkb = S / 64;
+  const int nkb = STRIDED ? (S + 63) / 64 : S / 64;
+  auto load_rows = [&](uint16_t* s, const uint16_t* g, int first, int ldg, int col0) {     // sequence rows first.. first+63
+    if constexpr (STRIDED) load_tile64<HD, true>(s, g, seq_row0 + static_cast<size_t>(first) * rs, ldg, col0, rs, S - first);
+    else load_tile64<HD>(s, g, seq_row0 + first, ldg, col0);
+  };
   zero_pads<HD>(sm, 6);
-  load_tile64<HD>(sQ, qkv, seq_row0 + q0, ld, h * HD);
-  load_tile64<HD>(sDO, d_o, seq_row0 + q0, D, h * HD);
-  load_tile64<HD>(sV, o, seq_row0 + q0, D, h * HD);            // O block, only for delta
-  load_tile64<HD>(sK, qkv, seq_row0, ld, D + h * HD);          // K block 0
+  load_rows(sQ, qkv, q0, ld, h * HD);
+  load_rows(sDO, d_o, q0, D, h * HD);
+  load_rows(sV, o, q0, D, h * HD);            // O block, only for delta
+  load_rows(sK, qkv, 0, ld, D + h * HD);      // K block 0
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
@@ -759,13 +798,14 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
   float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
   for (int kb = 0; kb < nkb; ++kb) {
     const uint16_t* cK = sK + (kb & 1) * G::TILE;
-    if (kb + 1 < nkb) load_tile64<HD>(sK + ((kb + 1) & 1) * G::TILE, qkv, seq_row0 + (kb + 1) * 64, ld, D + h * HD);
+    if (kb + 1 < nkb) load_rows(sK + ((kb + 1) & 1) * G::TILE, qkv, (kb + 1) * 64, ld, D + h * HD);
     else {                                     // last block of pass 1: start pass 2's first K / V block (V buffer 0 held O, now consumed)
-      if (nkb > 1) load_tile64<HD>(sK + ((kb + 1) & 1) * G::TILE, qkv, seq_row0, ld, D + h * HD);
+      if (nkb > 1) load_rows(sK + ((kb + 1) & 1) * G::TILE, qkv, 0, ld, D + h * HD);
     }
     cp_async_commit();
     float acc[8][4] = {};
     mm_a_tileT<BF16, HD>(acc, sQ, warp * 16, cK);
+    if constexpr (STRIDED) { if (S - kb * 64 < 64) mask_keys(acc, S - kb * 64); }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       float m = mx[hh];
@@ -789,7 +829,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
     t += __shfl_xor_sync(0xffffffffu, t, 1);
     t += __shfl_xor_sync(0xffffffffu, t, 2);
     l2[hh] = mx[hh] + log2f(t);
-    if ((lane & 3) == 0) {
+    if ((lane & 3) == 0 && (!STRIDED || q0 + r_lo + hh * 8 < S)) {
       const size_t idx = (static_cast<size_t>(seq) * heads + h) * S + q0 + r_lo + hh * 8;
       lse[idx] = l2[hh];
       delta[idx] = dl[hh];
@@ -797,17 +837,21 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
   }
   // ---- pass 2.  K block 0 sits in K buffer (nkb & 1) when nkb > 1 (prefetched above), else still in buffer 0.
   const int kbase = nkb > 1 ? (nkb & 1) : 0;
-  load_tile64<HD>(sV + kbase * G::TILE, qkv, seq_row0, ld, 2 * D + h * HD);
+  load_rows(sV + kbase * G::TILE, qkv, 0, ld, 2 * D + h * HD);
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  const float scale = scale_log2 * 0.6931471805599453f;
+  // fp16 and STRIDED keep the softmax scale out of the 16-bit dS operand and apply it to the fp32 dQ / dK at the end: dS of a
+  // mean loss over a whole video is small enough that another factor hd^-1/2 pushes many values into fp16's subnormal range
+  // (bf16 has the exponent range; its spatial instances keep the original order of operations)
+  constexpr bool DEFER = STRIDED || !BF16;
+  const float scale = DEFER ? 1.0f : scale_log2 * 0.6931471805599453f;
   float dq[G::NT][4] = {};
   for (int kb = 0; kb < nkb; ++kb) {
     const int cur = (kbase + kb) & 1, nxt = cur ^ 1;
     if (kb + 1 < nkb) {
-      load_tile64<HD>(sK + nxt * G::TILE, qkv, seq_row0 + (kb + 1) * 64, ld, D + h * HD);
-      load_tile64<HD>(sV + nxt * G::TILE, qkv, seq_row0 + (kb + 1) * 64, ld, 2 * D + h * HD);
+      load_rows(sK + nxt * G::TILE, qkv, (kb + 1) * 64, ld, D + h * HD);
+      load_rows(sV + nxt * G::TILE, qkv, (kb + 1) * 64, ld, 2 * D + h * HD);
     }
     cp_async_commit();
     const uint16_t* cK = sK + cur * G::TILE;
@@ -815,6 +859,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
     float s_acc[8][4] = {}, p_acc[8][4] = {};
     mm_a_tileT<BF16, HD>(s_acc, sQ, warp * 16, cK);
     mm_a_tileT<BF16, HD>(p_acc, sDO, warp * 16, cV);
+    if constexpr (STRIDED) { if (S - kb * 64 < 64) mask_keys(s_acc, S - kb * 64); }     // P = exp2(-inf) = 0 there
 #pragma unroll
     for (int n = 0; n < 8; ++n)
 #pragma unroll
@@ -829,16 +874,26 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const uint16_t* __rest
     cp_async_wait<0>();
     __syncthreads();
   }
-  store_rows<BF16, HD>(dqkv, seq_row0 + q0, ld, h * HD, dq, warp * 16, 64);
+  if constexpr (DEFER) {
+    const float sc = scale_log2 * 0.6931471805599453f;
+#pragma unroll
+    for (int n = 0; n < G::NT; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) dq[n][e] *= sc;
+  }
+  if constexpr (STRIDED) store_rows<BF16, HD, true>(dqkv, seq_row0 + static_cast<size_t>(q0) * rs, ld, h * HD, dq, warp * 16, S - q0, rs);
+  else store_rows<BF16, HD>(dqkv, seq_row0 + q0, ld, h * HD, dq, warp * 16, 64);
 }
 
 // Kernel B: one CTA = 64 keys of one (sequence, head); loops over the query blocks with the statistics of kernel A.
 // S^T = K Q^T so that the warp's accumulator rows are keys: P^T and dS^T are then directly the A operands of
 // dV = P^T dO and dK = dS^T Q.  Q / dO blocks (and their statistics) are double-buffered with cp.async.
-template <bool BF16, int HD>
+// STRIDED (see kernel A): queries at or beyond S are zero rows with lse = +inf and delta = 0, so their P and dS are exactly 0;
+// key rows at or beyond S are zero and never stored.
+template <bool BF16, int HD, bool STRIDED = false>
 __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ d_o,
                                                            uint16_t* __restrict__ dqkv, const float* __restrict__ lse,
-                                                           const float* __restrict__ delta, int S, int heads, float scale_log2) {
+                                                           const float* __restrict__ delta, int S, int heads, float scale_log2, int rs) {
   using G = AB<HD>;
   extern __shared__ __align__(16) uint16_t sm[];
   uint16_t* sK = sm;
@@ -850,24 +905,36 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const uint16_t* __res
   const int kb = blockIdx.x, h = blockIdx.y, seq = blockIdx.z;
   const int D = heads * HD, ld = 3 * D;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const size_t seq_row0 = static_cast<size_t>(seq) * S;
+  const size_t seq_row0 = STRIDED ? static_cast<size_t>(seq / rs) * S * rs + seq % rs : static_cast<size_t>(seq) * S;
   const size_t stat0 = (static_cast<size_t>(seq) * heads + h) * S;
   const int k0 = kb * 64;
-  const int nqb = S / 64;
+  const int nqb = STRIDED ? (S + 63) / 64 : S / 64;
+  auto load_rows = [&](uint16_t* s, const uint16_t* g, int first, int ldg, int col0) {
+    if constexpr (STRIDED) load_tile64<HD, true>(s, g, seq_row0 + static_cast<size_t>(first) * rs, ldg, col0, rs, S - first);
+    else load_tile64<HD>(s, g, seq_row0 + first, ldg, col0);
+  };
   auto load_q = [&](int qb, int buf) {
-    load_tile64<HD>(sQ + buf * G::TILE, qkv, seq_row0 + qb * 64, ld, h * HD);
-    load_tile64<HD>(sDO + buf * G::TILE, d_o, seq_row0 + qb * 64, D, h * HD);
-    if (threadIdx.x < 16) cp_async16(sL + buf * 64 + threadIdx.x * 4, lse + stat0 + qb * 64 + threadIdx.x * 4);
-    else if (threadIdx.x < 32) cp_async16(sD + buf * 64 + (threadIdx.x - 16) * 4, delta + stat0 + qb * 64 + (threadIdx.x - 16) * 4);
+    load_rows(sQ + buf * G::TILE, qkv, qb * 64, ld, h * HD);
+    load_rows(sDO + buf * G::TILE, d_o, qb * 64, D, h * HD);
+    if constexpr (STRIDED) {             // S need not be a multiple of 4: one float per thread
+      const int t = threadIdx.x & 63, qi = qb * 64 + t;
+      float* dst = (threadIdx.x < 64 ? sL : sD) + buf * 64 + t;
+      if (qi < S) cp_async4(dst, (threadIdx.x < 64 ? lse : delta) + stat0 + qi);
+      else *dst = threadIdx.x < 64 ? INFINITY : 0.f;
+    } else {
+      if (threadIdx.x < 16) cp_async16(sL + buf * 64 + threadIdx.x * 4, lse + stat0 + qb * 64 + threadIdx.x * 4);
+      else if (threadIdx.x < 32) cp_async16(sD + buf * 64 + (threadIdx.x - 16) * 4, delta + stat0 + qb * 64 + (threadIdx.x - 16) * 4);
+    }
   };
   zero_pads<HD>(sm, 6);
-  load_tile64<HD>(sK, qkv, seq_row0 + k0, ld, D + h * HD);
-  load_tile64<HD>(sV, qkv, seq_row0 + k0, ld, 2 * D + h * HD);
+  load_rows(sK, qkv, k0, ld, D + h * HD);
+  load_rows(sV, qkv, k0, ld, 2 * D + h * HD);
   load_q(0, 0);
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  const float scale = scale_log2 * 0.6931471805599453f;
+  constexpr bool DEFER = STRIDED || !BF16;        // softmax scale applied to the fp32 dK at the end (see kernel A)
+  const float scale = DEFER ? 1.0f : scale_log2 * 0.6931471805599453f;
   float dk[G::NT][4] = {}, dv[G::NT][4] = {};
   for (int qb = 0; qb < nqb; ++qb) {
     const int cur = qb & 1;
@@ -897,8 +964,21 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const uint16_t* __res
     cp_async_wait<0>();
     __syncthreads();
   }
-  store_rows<BF16, HD>(dqkv, seq_row0 + k0, ld, D + h * HD, dk, warp * 16, 64);
-  store_rows<BF16, HD>(dqkv, seq_row0 + k0, ld, 2 * D + h * HD, dv, warp * 16, 64);
+  if constexpr (DEFER) {
+    const float sc = scale_log2 * 0.6931471805599453f;
+#pragma unroll
+    for (int n = 0; n < G::NT; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) dk[n][e] *= sc;
+  }
+  if constexpr (STRIDED) {
+    const size_t r0 = seq_row0 + static_cast<size_t>(k0) * rs;
+    store_rows<BF16, HD, true>(dqkv, r0, ld, D + h * HD, dk, warp * 16, S - k0, rs);
+    store_rows<BF16, HD, true>(dqkv, r0, ld, 2 * D + h * HD, dv, warp * 16, S - k0, rs);
+  } else {
+    store_rows<BF16, HD>(dqkv, seq_row0 + k0, ld, D + h * HD, dk, warp * 16, 64);
+    store_rows<BF16, HD>(dqkv, seq_row0 + k0, ld, 2 * D + h * HD, dv, warp * 16, 64);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ attention backward (temporal)
@@ -1413,21 +1493,23 @@ int launch_ln_modulate_bwd(const void* dh16, const float* x, const float* scale,
 #undef LNB
 }
 
-template <bool BF16, int HD>
-static int attn_bwd_spatial(const uint16_t* qkv, const uint16_t* o, const uint16_t* d_o, uint16_t* dqkv, float* lse, float* delta,
-                            int nseq, int S, int heads, cudaStream_t stream) {
+// Spatial sequences (STRIDED = false): nseq = batch * frames sequences of S = tokens consecutive rows, S % 64 == 0.
+// Temporal sequences (STRIDED = true): nseq = batch * tokens sequences of S = frames rows at stride rs = tokens.
+template <bool BF16, int HD, bool STRIDED = false>
+static int attn_bwd_two_pass(const uint16_t* qkv, const uint16_t* o, const uint16_t* d_o, uint16_t* dqkv, float* lse, float* delta,
+                            int nseq, int S, int heads, cudaStream_t stream, int rs = 1) {
   using G = AB<HD>;
-  auto ka = attn_bwd_dq_kernel<BF16, HD>;
-  auto kb = attn_bwd_dkv_kernel<BF16, HD>;
+  auto ka = attn_bwd_dq_kernel<BF16, HD, STRIDED>;
+  auto kb = attn_bwd_dkv_kernel<BF16, HD, STRIDED>;
   const size_t smem_a = static_cast<size_t>(6) * G::TILE * 2;
   const size_t smem_b = smem_a + 256 * sizeof(float);
   B200_SET_SMEM_ONCE(ka, static_cast<int>(smem_a));
   B200_SET_SMEM_ONCE(kb, static_cast<int>(smem_b));
   const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(HD));
-  dim3 grid(S / 64, heads, nseq);
-  ka<<<grid, 128, smem_a, stream>>>(qkv, o, d_o, dqkv, lse, delta, S, heads, scale_log2);
+  dim3 grid((S + 63) / 64, heads, nseq);
+  ka<<<grid, 128, smem_a, stream>>>(qkv, o, d_o, dqkv, lse, delta, S, heads, scale_log2, rs);
   B200_CHECK_CUDA(cudaGetLastError());
-  kb<<<grid, 128, smem_b, stream>>>(qkv, d_o, dqkv, lse, delta, S, heads, scale_log2);
+  kb<<<grid, 128, smem_b, stream>>>(qkv, d_o, dqkv, lse, delta, S, heads, scale_log2, rs);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;
 }
@@ -1438,6 +1520,21 @@ int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* 
   B200_REQUIRE(ALIGNED16(qkv) && ALIGNED16(o) && ALIGNED16(d_o) && ALIGNED16(dqkv), B200_ERR_ALIGN, "attention_bwd: pointers must be 16-byte aligned");
   const uint16_t *q = static_cast<const uint16_t*>(qkv), *oo = static_cast<const uint16_t*>(o), *g = static_cast<const uint16_t*>(d_o);
   uint16_t* dq = static_cast<uint16_t*>(dqkv);
+  if (temporal && frames > 16) {                  // 17..128 frames: the two-kernel tensor-core backward over strided rows
+    B200_REQUIRE(frames <= 128 && (head_dim == 64 || head_dim == 72), B200_ERR_UNSUPPORTED,
+                 "attention_bwd: temporal sequences of 17..128 frames need head_dim 64 or 72 (got %d frames, head_dim %d)", frames, head_dim);
+    B200_REQUIRE(stats != nullptr && ALIGNED16(stats), B200_ERR_ALIGN, "attention_bwd: stats workspace missing");
+    const int nseq = batch * tokens;
+    B200_REQUIRE(nseq <= 65535 && heads <= 65535, B200_ERR_UNSUPPORTED, "attention_bwd: batch * tokens = %d sequences exceed the grid's z extent", nseq);
+    float* lse = stats;
+    float* delta = stats + static_cast<size_t>(nseq) * heads * frames;
+    if (head_dim == 72) {
+      if (bf16) return attn_bwd_two_pass<true, 72, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
+      return attn_bwd_two_pass<false, 72, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
+    }
+    if (bf16) return attn_bwd_two_pass<true, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
+    return attn_bwd_two_pass<false, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
+  }
   if (temporal) {
     B200_REQUIRE(frames <= 16 && head_dim % 8 == 0 && head_dim <= 128, B200_ERR_UNSUPPORTED, "attention_bwd: temporal sequences of <= 16 frames, head_dim %% 8 == 0 (got %d, %d)", frames, head_dim);
     if (head_dim == 64 || head_dim == 72) {       // tensor-core kernel: one warp per (b, n, head)
@@ -1473,11 +1570,11 @@ int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* 
   float* lse = stats;
   float* delta = stats + static_cast<size_t>(nseq) * heads * tokens;
   if (head_dim == 72) {
-    if (bf16) return attn_bwd_spatial<true, 72>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
-    return attn_bwd_spatial<false, 72>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
+    if (bf16) return attn_bwd_two_pass<true, 72>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
+    return attn_bwd_two_pass<false, 72>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
   }
-  if (bf16) return attn_bwd_spatial<true, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
-  return attn_bwd_spatial<false, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
+  if (bf16) return attn_bwd_two_pass<true, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
+  return attn_bwd_two_pass<false, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
 }
 
 int launch_ada_outer(const float* dmod, long long dmod_bs, const void* sc16, float* dW, int batch, int NA, int dim, int bf16, cudaStream_t stream) {

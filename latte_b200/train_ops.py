@@ -166,7 +166,9 @@ class NativeOps:
         self._cuda(qkv, o, do)
         D = o.shape[1]
         dqkv = torch.empty_like(qkv)
-        stats = None if temporal else torch.empty(2 * B * Fr * H * N, dtype=torch.float32, device=qkv.device)
+        # row statistics (lse, delta) of the two-kernel backward: spatial sequences and temporal ones longer than 16 frames;
+        # the <= 16-frame temporal kernel keeps them in shared memory
+        stats = None if temporal and Fr <= 16 else torch.empty(2 * B * Fr * H * N, dtype=torch.float32, device=qkv.device)
         with torch.cuda.device(qkv.device):
             rc = _lib.load().b200_attention_bwd(qkv.data_ptr(), o.data_ptr(), do.data_ptr(), dqkv.data_ptr(),
                                                 stats.data_ptr() if stats is not None else None, B, Fr, N, H, D // H, self.dt,
