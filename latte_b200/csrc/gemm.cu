@@ -15,12 +15,17 @@
 //                   stage; a stage is full when this CTA's A bytes and BOTH W halves have landed on its "full" barrier.
 //                   It waits only on "empty" and keeps every stage in flight, through the consumers' epilogues.
 //   warpgroups 1-2  the consumers: wgmma (64 x BN x 16, fp32 accumulators in registers), one 64-row half of the tile each,
-//                   then the epilogue straight from the accumulator registers; they wait only on "full", and a stage is
-//                   released with one arrival per warpgroup on the "empty" barriers of BOTH CTAs (the peer's next
-//                   multicast writes into it)
+//                   then the epilogue; they wait only on "full", and a stage is released with one arrival per warpgroup
+//                   on the "empty" barriers of BOTH CTAs (the peer's next multicast writes into it)
 //
-// Residual epilogue: every element of x is owned by one thread and updated in place (x += gate * (acc + bias) (+ row_add)),
-// once per GEMM -- or, for the stream-K tiles of the last waves, once per K segment in k order (TileSched below).
+// Epilogue: the consumers never write global memory themselves.  Each warpgroup moves its 64 rows of the tile, one column
+// chunk at a time, into one of its two 64-row x 128-byte staging buffers (128B-swizzled, the layout of a SW128 tensor map),
+// and one thread hands the chunk to TMA; the warpgroup goes straight on to the next chunk and then the next tile's MMAs
+// while the bytes drain.  TMA clips rows past M and columns past N.
+//   16-bit outputs:  64-column chunks, stmatrix into the buffer, cp.async.bulk.tensor store
+//   residual:        32-column fp32 chunks of the increment gate * (acc + bias) (+ row_add); x is never loaded: a
+//                    cp.reduce.async.bulk.tensor .add folds the chunk into the fp32 residual stream in L2, once per GEMM --
+//                    or, for the stream-K tiles of the last waves, once per K segment in k order (TileSched below).
 #include <cstdio>
 #include "common.h"
 #include "ptx.cuh"
@@ -40,20 +45,26 @@ constexpr int kThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1-2: MM
 constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
 
+// epilogue staging buffer: 64 rows x 128 bytes (32 fp32 or 64 16-bit columns), two per consumer warpgroup
+constexpr int kEpiBufBytes = 64 * 128;
+
 template <int BN, int EPI>
 struct Cfg {
   static constexpr bool RESID = EPI == B200_EPI_GATE_RESIDUAL;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;                       // the whole W tile (both CTAs' halves)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int EPI_BYTES = 2 * 2 * kEpiBufBytes;            // 2 consumer warpgroups x 2 buffers = 32 KiB
   static constexpr int BAR_BYTES = 256;
-  static constexpr int STAGES_FIT = (232448 - BAR_BYTES - 1024) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // BN 256: 4, 192: 5, 128: 7
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int STAGES_FIT = (232448 - EPI_BYTES - BAR_BYTES - 1024) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // BN 256: 4, 192: 4, 128: 6
+  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;             // 1 KiB aligned: the buffers keep the swizzle phase
+  static constexpr int BAR_OFF = EPI_OFF + EPI_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFF + BAR_BYTES + 1024;    // +1024: manual 1 KiB alignment of the base
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1 KiB alignment");
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
   static_assert(2 * STAGES <= BAR_BYTES / 8, "barrier area too small");
+  static_assert(BN % 64 == 0, "the 16-bit epilogue works in 64-column chunks");
 };
 
 struct GemmDev {
@@ -155,11 +166,8 @@ __device__ __forceinline__ float resid_delta(float acc, float b, float gt, float
   return has_ra ? __fadd_rn(dv, ra) : dv;
 }
 
-// column groups per batch of epilogue loads in the full-tile paths: all loads of a chunk are issued before its first use
-constexpr int kEpiChunk = 8;
-// ends a chunk: keeps the compiler (ptxas included: bar.warp.sync orders memory) from hoisting the next chunk's loads above
-// it, which would hold the loads of the whole tile in registers next to the accumulators and spill
-__device__ __forceinline__ void epi_chunk_fence() { __syncwarp(); }
+// named barrier of consumer warpgroup wg (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void epi_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5 x (1 + tanh(u)),  u = sqrt(2/pi) (x + 0.044715 x^3).  ONE MUFU op per element (tanh.approx, rel. error 2^-11,
@@ -179,11 +187,12 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 // an injected empty wgmma group, which turns wgmma_wait<1> into a full drain.
 template <int BN, int EPI, bool BF16, int MN>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmDev p) {
+  // tmC: the output, fp32 resid [M, N] (box 32 x 64) or 16-bit out16 [M, N] (box 64 x 64); tmC2: out16b (GELU_BOTH only)
   using C = Cfg<BN, EPI>;
   constexpr int TA = MN & 1, TB = MN >> 1;
   static_assert(MN == 0 || MN == 2 || MN == 3, "operand layouts: 0 forward, 2 dgrad, 3 wgrad");
-  static_assert((BN / 8) % kEpiChunk == 0, "the epilogue chunks must tile the 8-column groups of a tile exactly");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
@@ -196,6 +205,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmC);
+    if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) tma_prefetch_desc(&tmC2);
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full[i], 1);    // this CTA's expect_tx arrival; the bytes of both W halves and of A complete it
       mbar_init(&empty[i], 4);   // one arrival per consumer warpgroup of BOTH CTAs (each W half lands in both)
@@ -275,6 +286,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
+    uint8_t* epi = smem + C::EPI_OFF;         // this CTA's four staging buffers; warpgroup wg owns 2 wg and 2 wg + 1
+    int ep = 0;                               // chunks this warpgroup has staged so far: chunk i uses buffer i % 2
     TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
     int tile, kb0, kb1;
     while (sched.next(tile, kb0, kb1)) {
@@ -308,167 +321,150 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         mbar_arrive_cluster(empty_peer + prev * 8);
       }
 
-      // accumulator fragment: thread (w4, g, cq) holds rows r0 = 16*w4 + g and r0 + 8 of its 64, columns 8j + 2cq + {0,1}
-      const int r0 = m0 + wg * 64 + w4 * 16 + g;
+      // accumulator fragment: thread (w4, g, cq) holds rows lr0 = 16*w4 + g and lr0 + 8 of its warpgroup's 64 (which start
+      // at row m0w of the matrix), columns 8j + 2cq + {0,1}: acc[4j + 2h + {0,1}] for row lr0 + 8h
+      const int m0w = m0 + wg * 64;
+      const int lr0 = w4 * 16 + g;
       if constexpr (C::RESID) {
-        // x += gate * (acc + bias) (+ row_add): every element belongs to one thread and receives one add per GEMM -- or,
-        // for stream-K tiles, one per segment in k order (the flag of the tile's rows of this warpgroup) -- so results
-        // are deterministic
+        // x += gate * (acc + bias) (+ row_add) without ever loading x: the increment goes to a staging buffer in 32-column
+        // chunks and TMA adds each chunk into x in L2.  Every element receives one add per GEMM -- or, for stream-K tiles,
+        // one per segment in k order (the flag of the tile's rows of this warpgroup) -- so results are deterministic.
         const bool first_seg = kb0 == 0;       // bias and row_add are added once per output element
         const bool partial = kb0 > 0 || kb1 < num_kb;
         unsigned long long* flag = nullptr;
         if (partial) flag = p.sk_flags + (static_cast<size_t>(tile - sched.full_waves * num_pairs) * 2 + rank) * 2 + wg;
-        if (kb0 > 0) {
-          if (te == 0) {
-            flag_wait(flag, static_cast<unsigned long long>(kb0));
-            // nobody else waits on this flag; the segment that completes the tile leaves it zero for the next launch
-            if (kb1 == num_kb) flag_release(flag, 0ull);
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-        }
+        bool ordered = kb0 == 0;               // issuing thread: may this segment add into x yet?
         const float* bias = (p.bias && first_seg) ? p.bias : nullptr;
-        const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
+        const float* gate_row[2];
+        const float* add_row[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          // rows past M are skipped per lane (M need not be a multiple of 8, so one warp can hold both kinds); the row
-          // pointers are formed from a clamped row and never dereferenced for such a lane
-          const bool row_ok = row < p.M;
-          if (BN > 192 && !row_ok) continue;   // no chunked path (and no fence) at BN = 256: skip the row outright
-          const int prow = row_ok ? row : p.M - 1;
-          const float* gate_row = p.gate + static_cast<long long>(prow / p.rows_per_batch) * p.gate_bs;
-          const float* add_row = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((prow / p.row_add_div) % p.row_add_period) * p.N : nullptr;
-          float* xrow = p.resid + static_cast<size_t>(prow) * p.N;
-          if (BN <= 192 && live == BN / 8) {
-            // whole tile inside N: the x loads of a chunk of column groups (HBM / L2 round trips) are all in flight before
-            // the chunk's first store, instead of one dependent round trip per column group; gate, bias and row_add are
-            // L1-resident after the first warp's touch.  Not at BN = 256: beside its 128 accumulators the batch spills.
-            // Every lane of the warp reaches each chunk fence (a __syncwarp): rows past M only predicate the memory accesses.
+          // a row past M computes an increment from a clamped row, and the reduce-add clips it
+          const int row = m0w + lr0 + 8 * h < p.M ? m0w + lr0 + 8 * h : p.M - 1;
+          gate_row[h] = p.gate + static_cast<long long>(row / p.rows_per_batch) * p.gate_bs;
+          add_row[h] = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((row / p.row_add_div) % p.row_add_period) * p.N : nullptr;
+        }
 #pragma unroll
-            for (int j0 = 0; j0 < BN / 8; j0 += kEpiChunk) {
-              float2 x[kEpiChunk];
+        for (int c = 0; c < BN / 32; ++c) {
+          if (n0 + 32 * c >= p.N) break;       // N % 32 == 0: a chunk lies wholly inside N or wholly past it
+          uint8_t* buf = epi + (2 * wg + (ep & 1)) * kEpiBufBytes;
+          const uint32_t buf_addr = smem_u32(buf);
 #pragma unroll
-              for (int j = 0; j < kEpiChunk; ++j)
-                if (row_ok) x[j] = *reinterpret_cast<const float2*>(xrow + n0 + 8 * (j0 + j) + 2 * cq);
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * c + jj, col = n0 + 8 * j + 2 * cq;
+            const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
-              for (int j = 0; j < kEpiChunk; ++j) {
-                if (!row_ok) continue;
-                const int col = n0 + 8 * (j0 + j) + 2 * cq;
-                const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
-                const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
-                const float2 ra = add_row ? __ldg(reinterpret_cast<const float2*>(add_row + col)) : make_float2(0.f, 0.f);
-                x[j].x = __fadd_rn(x[j].x, resid_delta(acc[4 * (j0 + j) + 2 * h], b2.x, gt.x, ra.x, add_row != nullptr));
-                x[j].y = __fadd_rn(x[j].y, resid_delta(acc[4 * (j0 + j) + 2 * h + 1], b2.y, gt.y, ra.y, add_row != nullptr));
-                *reinterpret_cast<float2*>(xrow + col) = x[j];
-              }
-              epi_chunk_fence();
-            }
-          } else if (row_ok) {
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-              if (j >= live) break;
-              const int col = n0 + 8 * j + 2 * cq;
-              const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
-              const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row + col));
-              const float2 ra = add_row ? __ldg(reinterpret_cast<const float2*>(add_row + col)) : make_float2(0.f, 0.f);
-              float2 x = *reinterpret_cast<const float2*>(xrow + col);
-              x.x = __fadd_rn(x.x, resid_delta(acc[4 * j + 2 * h], b2.x, gt.x, ra.x, add_row != nullptr));
-              x.y = __fadd_rn(x.y, resid_delta(acc[4 * j + 2 * h + 1], b2.y, gt.y, ra.y, add_row != nullptr));
-              *reinterpret_cast<float2*>(xrow + col) = x;
+            for (int h = 0; h < 2; ++h) {
+              const float2 gt = __ldg(reinterpret_cast<const float2*>(gate_row[h] + col));
+              const float2 ra = add_row[h] ? __ldg(reinterpret_cast<const float2*>(add_row[h] + col)) : make_float2(0.f, 0.f);
+              const float d0 = resid_delta(acc[4 * j + 2 * h], b2.x, gt.x, ra.x, add_row[h] != nullptr);
+              const float d1 = resid_delta(acc[4 * j + 2 * h + 1], b2.y, gt.y, ra.y, add_row[h] != nullptr);
+              // buffer row lr0 + 8h is 128 bytes; its 16-byte units are XOR-swizzled by the row % 8 (= g), as SW128 TMA reads them
+              st_shared_f2(buf_addr + (lr0 + 8 * h) * 128 + (((2 * jj + (cq >> 1)) ^ g) << 4) + 8 * (cq & 1), d0, d1);
             }
           }
+          fence_proxy_async_smem();            // the writes above -> visible to TMA
+          epi_bar(wg);
+          if (te == 0) {
+            if (!ordered) {
+              // continuing segment: acquire the previous segment's release (it follows that segment's completed adds) ...
+              flag_wait(flag, static_cast<unsigned long long>(kb0));
+              fence_proxy_async_global();      // ... and order our reduce-adds (async proxy) after the acquire
+              if (kb1 == num_kb) flag_release(flag, 0ull);   // nobody else waits on it; left zero for the next launch
+              ordered = true;
+            }
+            tma_reduce_add_2d(&tmC, buf, n0 + 32 * c, m0w);
+            tma_store_commit();
+            tma_store_wait_read<1>();          // the previous chunk has been read out of the other buffer ...
+          }
+          epi_bar(wg);                         // ... which may now be rewritten
+          ++ep;
         }
-        if (partial && kb1 < num_kb) {
-          __threadfence();                     // this segment's adds are visible ...
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-          if (te == 0) flag_release(flag, static_cast<unsigned long long>(kb1));   // ... the next segment may add
+        if (partial && kb1 < num_kb && te == 0) {
+          tma_store_wait_all<0>();             // this segment's adds have been performed in x ...
+          fence_proxy_async_global();          // ... and are ordered before the generic-proxy release:
+          flag_release(flag, static_cast<unsigned long long>(kb1));   // the next segment may add
         }
       } else {
-        bool done = false;
-        if constexpr (EPI == B200_EPI_BIAS || EPI == B200_EPI_BIAS_GELU) {
-          if (p.N - n0 >= BN) {
-            // whole tile inside N (bias / bias + GELU epilogues): a chunk's bias loads are issued together and shared by both
-            // row halves, instead of one dependent load before every store
-            const bool row_ok[2] = {r0 < p.M, r0 + 8 < p.M};
-            uint32_t* orow[2];
+        // 16-bit output(s) in 64-column chunks, each value rounded exactly as a direct store would round it, then stmatrix
+        // into the swizzled buffer: an 8x8 matrix is 8 rows x one 16-byte unit, the rows in 8 different bank groups
+        constexpr bool TWO = EPI == B200_EPI_BIAS_GELU_BOTH;   // out16 and out16b: both buffers per chunk
+        const int mi = lane >> 3;                               // the matrix whose row this lane addresses
+        const int lrow = w4 * 16 + (lane & 7) + 8 * (mi & 1);
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-              orow[h] = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(r0 + 8 * h) * p.N);
+        for (int c = 0; c < BN / 64; ++c) {
+          if (n0 + 64 * c >= p.N) break;       // N % 32 == 0: the last chunk may be half inside N; TMA clips the rest
+          uint8_t* buf = epi + (2 * wg + (TWO ? 0 : (ep & 1))) * kEpiBufBytes;
+          const uint32_t row_addr = smem_u32(buf) + lrow * 128;
 #pragma unroll
-            for (int j0 = 0; j0 < BN / 8; j0 += kEpiChunk) {
-              float2 b[kEpiChunk];
+          for (int jp = 0; jp < 4; ++jp) {     // column groups j = 8c + 2jp + q, q = 0, 1: matrix 2q + h holds rows lr0 + 8h
+            uint32_t v[4], vb[4];
 #pragma unroll
-              for (int j = 0; j < kEpiChunk; ++j)
-                b[j] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * (j0 + j) + 2 * cq)) : make_float2(0.f, 0.f);
+            for (int q = 0; q < 2; ++q) {
+              const int j = 8 * c + 2 * jp + q, col = n0 + 8 * j + 2 * cq;
+              const bool col_ok = col < p.N;
+              const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                if (!row_ok[h]) continue;
-#pragma unroll
-                for (int j = 0; j < kEpiChunk; ++j) {
-                  const int col = n0 + 8 * (j0 + j) + 2 * cq;
-                  float f0 = acc[4 * (j0 + j) + 2 * h], f1 = acc[4 * (j0 + j) + 2 * h + 1];
-                  if (p.bias) { f0 += b[j].x; f1 += b[j].y; }
-                  if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
-                  orow[h][col / 2] = pack2<BF16>(f0, f1);
+                float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                if (p.bias) { f0 += b2.x; f1 += b2.y; }
+                if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+                uint32_t val = pack2<BF16>(f0, f1);
+                if constexpr (EPI == B200_EPI_BIAS_ADD16 || EPI == B200_EPI_BIAS_MUL16 || EPI == B200_EPI_MUL_GELUGRAD16) {
+                  const int row = m0w + lr0 + 8 * h;
+                  const uint32_t side = (row < p.M && col_ok)
+                      ? __ldg(reinterpret_cast<const uint32_t*>(p.add16) + (static_cast<size_t>(row) * p.N + col) / 2) : 0u;
+                  const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(side);
+                  // + shortcut, both already rounded to 16 bits like the reference
+                  if constexpr (EPI == B200_EPI_BIAS_ADD16) val = pack2<BF16>(a.x + r.x, a.y + r.y);
+                  // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
+                  if constexpr (EPI == B200_EPI_BIAS_MUL16) val = pack2<BF16>(a.x * r.x, a.y * r.y);
+                  // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
+                  if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
                 }
+                if constexpr (TWO) {           // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
+                  const float2 a = unpack2<BF16>(val);
+                  vb[2 * q + h] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
+                }
+                v[2 * q + h] = val;
               }
-              epi_chunk_fence();
             }
-            done = true;
+            // this lane's row holds column group 2jp + (mi >> 1) in 16-byte unit (2jp + (mi >> 1)) ^ (lrow % 8)
+            const uint32_t unit = ((2 * jp + (mi >> 1)) ^ (lane & 7)) << 4;
+            stmatrix_x4(row_addr + unit, v[0], v[1], v[2], v[3]);
+            if constexpr (TWO) stmatrix_x4(row_addr + kEpiBufBytes + unit, vb[0], vb[1], vb[2], vb[3]);
           }
-        }
-        if (!done) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = r0 + 8 * h;
-            if (row >= p.M) continue;
-            uint32_t* orow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out16) + static_cast<size_t>(row) * p.N);
-            const int live = (p.N - n0) / 8 < BN / 8 ? (p.N - n0) / 8 : BN / 8;   // 8-column groups inside N (N % 32 == 0)
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-              if (j >= live) break;
-              const int col = n0 + 8 * j + 2 * cq;
-              float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-              if (p.bias) {
-                const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-                f0 += b.x; f1 += b.y;
-              }
-              if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
-              uint32_t val = pack2<BF16>(f0, f1);
-              const size_t off = (static_cast<size_t>(row) * p.N + col) / 2;
-              if constexpr (EPI == B200_EPI_BIAS_MUL16) {   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
-                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-                val = pack2<BF16>(a.x * r.x, a.y * r.y);
-              }
-              if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) {   // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
-                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-                val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
-              }
-              if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) {   // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
-                const float2 a = unpack2<BF16>(val);
-                reinterpret_cast<uint32_t*>(p.out16b)[off] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
-              }
-              if constexpr (EPI == B200_EPI_BIAS_ADD16) {   // + shortcut, both already rounded to 16 bits like the reference
-                const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(__ldg(reinterpret_cast<const uint32_t*>(p.add16) + off));
-                val = pack2<BF16>(a.x + r.x, a.y + r.y);
-              }
-              orow[col / 2] = val;
-            }
+          fence_proxy_async_smem();            // the writes above -> visible to TMA
+          epi_bar(wg);
+          if (te == 0) {
+            tma_store_2d(&tmC, buf, n0 + 64 * c, m0w);
+            if constexpr (TWO) tma_store_2d(&tmC2, buf + kEpiBufBytes, n0 + 64 * c, m0w);
+            tma_store_commit();
+            // TWO rewrites both buffers every chunk; otherwise the previous chunk has been read out of the other buffer ...
+            if constexpr (TWO) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
           }
+          epi_bar(wg);                         // ... which may now be rewritten
+          ++ep;
         }
       }
     }
+    // every store / reduce-add of this warpgroup has been performed before the CTA retires, so the writes are complete with
+    // the grid, as a PDL-launched successor's griddepcontrol.wait expects
+    if (te == 0) tma_store_wait_all<0>();
   }
 
   cluster_sync_all();   // the peer may still multicast into our smem / arrive on our barriers until it is done too
 }
 
+// the kernel's four tensor maps: operands A and W, output (resid or out16) and second output (out16b)
+struct GemmMaps { CUtensorMap a, b, c, c2; };
+
 template <int BN, int EPI, bool BF16, int MN>
-int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t stream) {
+int launch_one(const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t stream) {
   using C = Cfg<BN, EPI>;
   auto kern = gemm_kernel<BN, EPI, BF16, MN>;
   B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tmA, tmB, p));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tm.a, tm.b, tm.c, tm.c2, p));
   return B200_OK;
 }
 
@@ -476,31 +472,30 @@ int launch_one(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p,
 // dgrad's bias / GELU-gradient with W stored [K, N], and wgrad's unit-gate accumulation with both operands transposed
 // (transposed operands take 128- or 256-wide tiles only).
 template <int BN, bool BF16>
-int launch_epi(int epi, int mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid, cudaStream_t s) {
+int launch_epi(int epi, int mn, const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t s) {
   if (mn == 0) {
     switch (epi) {
-      case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16, 0>(tmA, tmB, p, grid, s);
-      case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 0>(tmA, tmB, p, grid, s);
+      case B200_EPI_BIAS: return launch_one<BN, B200_EPI_BIAS, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_BIAS_GELU: return launch_one<BN, B200_EPI_BIAS_GELU, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_GATE_RESIDUAL: return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16, 0>(tm, p, grid, s);
+      case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 0>(tm, p, grid, s);
     }
   }
   if constexpr (BN != 192) {
-    if (mn == 2 && epi == B200_EPI_BIAS) return launch_one<BN, B200_EPI_BIAS, BF16, 2>(tmA, tmB, p, grid, s);
-    if (mn == 2 && epi == B200_EPI_MUL_GELUGRAD16) return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 2>(tmA, tmB, p, grid, s);
-    if (mn == 3 && epi == B200_EPI_GATE_RESIDUAL) return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 3>(tmA, tmB, p, grid, s);
+    if (mn == 2 && epi == B200_EPI_BIAS) return launch_one<BN, B200_EPI_BIAS, BF16, 2>(tm, p, grid, s);
+    if (mn == 2 && epi == B200_EPI_MUL_GELUGRAD16) return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 2>(tm, p, grid, s);
+    if (mn == 3 && epi == B200_EPI_GATE_RESIDUAL) return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 3>(tm, p, grid, s);
   }
   set_error("gemm: epilogue %d with operand layout %d and block_n %d is not built", epi, mn, BN);
   return B200_ERR_UNSUPPORTED;
 }
 
 template <int BN>
-int launch_bn(int bf16, int epi, int mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, int grid,
-              cudaStream_t s) {
-  return bf16 ? launch_epi<BN, true>(epi, mn, tmA, tmB, p, grid, s) : launch_epi<BN, false>(epi, mn, tmA, tmB, p, grid, s);
+int launch_bn(int bf16, int epi, int mn, const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t s) {
+  return bf16 ? launch_epi<BN, true>(epi, mn, tm, p, grid, s) : launch_epi<BN, false>(epi, mn, tm, p, grid, s);
 }
 
 constexpr int kStreamKMinKb = 32;          // K / 64 below which the split costs more than the idle tail it removes
@@ -516,6 +511,10 @@ int pick_block_n(int M, int N, int K, bool resid, int sms) {
   // minimise waves x per-tile time.  A tile's cost is modelled by the operand bytes a CTA receives per k-block, A plus
   // its multicast half of W: 128 + BN/2.
   // Where the last wave is streamed along K (residual epilogue, long K) there is no wave rounding.
+  // Re-measured with the TMA epilogue on 132 SMs (DESIGN §6): this picks the fastest width for proj and fc1, and widths
+  // 4-6 % slower than 192 for QKV and fc2.  No per-tile cost independent of the SM count picks 192 for QKV on 132 SMs
+  // but keeps 256 on 148 (QKV at 256 / 192: 7 / 9 waves on 132 SMs, 7 / 8 on 148), and the 148-SM choices are kept as
+  // tests/test_schedule.py states them, so the rule is unchanged.
   if (N <= 128) return 128;   // narrow outputs (e.g. the VAE's 3-channel conv_out padded to 32): smallest tile that covers N
   static const bool no_sk = env_int("B200_GEMM_NO_STREAMK", 0) != 0;
   const bool sk = resid && !no_sk && K / BK >= streamk_min_kb();
@@ -633,7 +632,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   const GemmPlan plan = plan_gemm(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, a.mn_major == 3);
   const int bn = plan.bn;
 
-  CUtensorMap tmA, tmB;
+  GemmMaps tm;
+  CUtensorMap& tmA = tm.a;
+  CUtensorMap& tmB = tm.b;
   int conv_bw = 0, conv_bh = 0;
   {
     if (a.conv_taps > 0) {
@@ -672,6 +673,21 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
       const uint32_t boxB[2] = {BK, static_cast<uint32_t>(bn / 2)};   // each CTA of the pair fetches half and multicasts it
       B200_TRY(make_tmap_16bit(&tmB, a.W, 2, dimsB, strB, boxB, TMAP_SW_128));
     }
+    // the output, [M, N] row-major: one 64-row x 128-byte box per staging buffer (32 fp32 or 64 16-bit columns); the
+    // alignment checks above and N % 32 == 0 give TMA its 16-byte base and row stride
+    const uint64_t dimsC[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
+    if (resid) {
+      const uint64_t strC[1] = {static_cast<uint64_t>(a.N) * 4};
+      const uint32_t boxC[2] = {32, 64};
+      B200_TRY(make_tmap(&tm.c, a.resid, 4, 2, dimsC, strC, boxC, TMAP_SW_128));
+      tm.c2 = tm.c;
+    } else {
+      const uint64_t strC[1] = {static_cast<uint64_t>(a.N) * 2};
+      const uint32_t boxC[2] = {64, 64};
+      B200_TRY(make_tmap_16bit(&tm.c, a.out16, 2, dimsC, strC, boxC, TMAP_SW_128));
+      if (a.epilogue == B200_EPI_BIAS_GELU_BOTH) B200_TRY(make_tmap_16bit(&tm.c2, a.out16b, 2, dimsC, strC, boxC, TMAP_SW_128));
+      else tm.c2 = tm.c;
+    }
   }
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
@@ -705,9 +721,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     p.sk_flags = p.streamk ? a.sk_flags : nullptr;
   }
   switch (bn) {
-    case 128: return launch_bn<128>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
-    case 192: return launch_bn<192>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
-    default: return launch_bn<256>(a.bf16, a.epilogue, a.mn_major, tmA, tmB, p, grid, stream);
+    case 128: return launch_bn<128>(a.bf16, a.epilogue, a.mn_major, tm, p, grid, stream);
+    case 192: return launch_bn<192>(a.bf16, a.epilogue, a.mn_major, tm, p, grid, stream);
+    default: return launch_bn<256>(a.bf16, a.epilogue, a.mn_major, tm, p, grid, stream);
   }
 }
 

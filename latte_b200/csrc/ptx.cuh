@@ -117,6 +117,9 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> visible to async proxy (wgmma/TMA)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
+// orders this thread's global-memory accesses through the generic proxy with those through the async proxy (TMA stores
+// and reductions), in both directions
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- TMA loads (tile mode, mbarrier completion)
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -194,6 +197,16 @@ __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const vo
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
                : "memory");
+}
+// 8-byte shared-memory store through a shared-window address (a generic pointer would give a generic ST)
+__device__ __forceinline__ void st_shared_f2(uint32_t saddr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
+}
+// four 8x8 16-bit matrices to shared memory: register i of lane (4g + q) holds row g, columns 2q, 2q + 1 of matrix i (the
+// wgmma / mma accumulator fragment once packed); lane l gives the address of row l % 8 of matrix l / 8 (16 bytes)
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
