@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 3
+#define B200_ABI_VERSION 4
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
 #else
@@ -42,8 +42,7 @@ enum {
 };
 enum { B200_FP16 = 0, B200_BF16 = 1 };
 enum { B200_EPI_BIAS = 0, B200_EPI_BIAS_GELU = 1, B200_EPI_GATE_RESIDUAL = 2, B200_EPI_BIAS_ADD16 = 3, B200_EPI_BIAS_MUL16 = 4,
-       B200_EPI_BIAS_GELU_BOTH = 5,   /* training fc1: out16 = acc + bias (kept for the backward), aux16 (written) = gelu_tanh(out16) */
-       B200_EPI_MUL_GELUGRAD16 = 6 }; /* training dgrad of fc2: out16 = acc * gelu_tanh'(aux16), aux16 = fc1's pre-activation (read)  */
+       B200_EPI_BIAS_GELU_BOTH = 5 }; /* training fc1: out16 = acc + bias (kept for the backward), aux16 (written) = gelu_tanh(out16) */
 
 /* Model geometry: the ctor arguments of reference `Latte` (models/latte.py:208-223). */
 typedef struct B200LatteShape {
@@ -372,11 +371,6 @@ B200_API int b200_linear(const void* A, const void* W, const float* bias, int M,
 B200_API int b200_attention(const void* qkv, void* out, int batch, int frames, int tokens, int heads, int head_dim,
                    int dtype, int temporal, void* stream);
 
-/* Attention-kernel selector, kept for ABI compatibility.  The sm_90a build has ONE attention forward kernel: 0 (default),
- * 2 and 3 (the kernel generations of earlier builds) are accepted and all select it; other values return
- * B200_ERR_UNSUPPORTED.                                                                                              */
-B200_API int b200_set_attention_impl(int impl);
-
 /* out16[r, :] = LayerNorm(x[r, :]; no affine, eps 1e-6) * (1 + scale[b]) + shift[b], b = r / rows_per_batch
  * — replaces norm1/norm2 + modulate (latte.py:28-29, 166-168, 179-180). x fp32 [rows, dim].          */
 B200_API int b200_ln_modulate(const float* x, const float* shift, const float* scale, int64_t mod_batch_stride,
@@ -394,18 +388,13 @@ B200_API int b200_ln_modulate(const float* x, const float* shift, const float* s
 B200_API int b200_wgrad(const void* dy16, const void* x16, const float* col_scale, float* dW, int rows, int n_out, int n_in,
                         int dtype, void* sk_flags, void* stream);
 /* dX16[rows, n_in] = dY16[rows, n_out] . W16[n_out, n_in] -- the input gradient of Y = X W^T with the weight in its nn.Linear
- * [out, in] layout (MN-major W operand: no transposed weight copy).  n_out % 64 == 0, n_in % 128 == 0.
- * gelu_u16 != NULL: X = gelu_tanh(U) and the result is the gradient w.r.t. U: dX * gelu_tanh'(U[rows, n_in]), fused in the epilogue
- * (the backward of timm Mlp's act between fc1 and fc2, latte.py:169-171).                                                     */
-B200_API int b200_dgrad(const void* dy16, const void* w16, const void* gelu_u16, void* dx16, int rows, int n_out, int n_in, int dtype,
-                        void* stream);
+ * [out, in] layout (MN-major W operand: no transposed weight copy).  n_out % 64 == 0, n_in % 128 == 0.                    */
+B200_API int b200_dgrad(const void* dy16, const void* w16, void* dx16, int rows, int n_out, int n_in, int dtype, void* stream);
 /* Training-mode fc1: u16 = A W^T + bias (kept for the backward) and a16 = gelu_tanh(u16) from the same epilogue.              */
 B200_API int b200_linear_gelu_both(const void* A, const void* W, const float* bias, int M, int N, int K, int dtype, void* u16, void* a16,
                                    void* stream);
 /* out16[cols, rows] = in16[rows, cols]^T (operands of shapes b200_wgrad / b200_dgrad do not take).                          */
 B200_API int b200_transpose16(const void* in16, void* out16, int rows, int cols, void* stream);
-/* fp32 master parameter [rows, cols] -> 16-bit copy and (out16_t != NULL) its transpose [cols, rows], one read.           */
-B200_API int b200_cast_transpose(const float* in, void* out16, void* out16_t, int rows, int cols, int dtype, void* stream);
 /* fp32 -> 16-bit elementwise (n % 4 == 0).                                                                                */
 /* The same for many tensors in ONE launch (all parameters at the start of a step).  table: device array of n_entries records
  * of four int64 {src fp32 pointer (16-byte aligned), dst 16-bit pointer (8-byte aligned), n4 = element count / 4, first_chunk}
@@ -426,13 +415,6 @@ B200_API int b200_cast16(const float* in, void* out16, int64_t n, int dtype, voi
  * (latte.py:357-358).                                                                                                     */
 B200_API int b200_gate_residual(const float* x, const void* m16, const float* gate, int64_t gate_batch_stride, int rows_per_batch,
                                 const float* row_add, int tokens, int frames, float* out, int rows, int dim, int dtype, void* stream);
-/* b200_gate_residual followed by b200_ln_modulate of its result, in one pass: x_out as above AND h16 = LayerNorm(x_out) * (1 +
- * scale[b]) + shift[b] (the next GEMM's operand; latte.py:179-180 across the two halves of a block / consecutive blocks).         */
-B200_API int b200_gate_residual_ln(const float* x, const void* m16, const float* gate, int64_t gate_batch_stride, const float* shift,
-                                   const float* scale, int64_t mod_batch_stride, int rows_per_batch, const float* row_add, int tokens, int frames,
-                                   float* x_out, void* h16, int rows, int dim, int dtype, void* stream);
-/* a16 = gelu_tanh(u16) (timm Mlp act, latte.py:169).                                                                      */
-B200_API int b200_gelu(const void* u16, void* a16, int64_t n, int dtype, void* stream);
 /* du16 = da16 * gelu_tanh'(u16); dbias[dim] (fp32) += column sums of du = fc1.bias gradient.  (Every reduction output of the
  * training passes ACCUMULATES: the caller zeroes its gradient buffers once per step, so no pass issues a memset.)          */
 B200_API int b200_gelu_bwd(const void* da16, const void* u16, void* du16, float* dbias, int rows, int dim, int dtype, void* stream);
@@ -449,8 +431,9 @@ B200_API int b200_ln_modulate_bwd(const void* dh16, const float* x, const float*
                                   float* dx, float* dshift, float* dscale, int64_t dmod_batch_stride, int rows, int dim, int dtype,
                                   void* stream);
 /* backward of b200_attention: dqkv16 [T, 3*heads*head_dim] from qkv16, o16 (its output) and do16.  Scores are recomputed on
- * mma.sync tensor cores (spatial: tokens % 64 == 0, head_dim 64 or 72; stats = 2 * batch*frames*heads*tokens floats of
- * scratch) or in shared memory (temporal: frames <= 16; stats unused).                                                     */
+ * mma.sync tensor cores; head_dim 64 or 72 at every frame count, other head dims return B200_ERR_UNSUPPORTED.
+ * Spatial: tokens % 64 == 0.  Temporal: 1..128 frames.  stats = 2 * batch*frames*heads*tokens floats of scratch (unused by
+ * temporal sequences of 16 frames or fewer).                                                                                */
 B200_API int b200_attention_bwd(const void* qkv16, const void* o16, const void* do16, void* dqkv16, float* stats, int batch,
                                 int frames, int tokens, int heads, int head_dim, int dtype, int temporal, void* stream);
 /* adaLN_modulation Linear on `batch` <= 8 conditioning rows (all blocks stacked, NA = depth*6*dim + 2*dim output features):

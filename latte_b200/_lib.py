@@ -10,11 +10,11 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buffer
 OK = 0
 FP16, BF16 = 0, 1
-EPI_BIAS, EPI_BIAS_GELU, EPI_GATE_RESIDUAL, EPI_BIAS_ADD16, EPI_BIAS_MUL16, EPI_BIAS_GELU_BOTH, EPI_MUL_GELUGRAD16 = 0, 1, 2, 3, 4, 5, 6
+EPI_BIAS, EPI_BIAS_GELU, EPI_GATE_RESIDUAL, EPI_BIAS_ADD16, EPI_BIAS_MUL16, EPI_BIAS_GELU_BOTH = 0, 1, 2, 3, 4, 5
 VAE_CONV3X3, VAE_CONV_T3, VAE_CONV_DOWN2 = 0, 1, 2
 ERR_NAMES = {-1: "SHAPE", -2: "DTYPE", -3: "ALIGN", -4: "ARCH", -5: "WORKSPACE", -6: "CUDA", -7: "UNSUPPORTED"}
 
@@ -121,7 +121,6 @@ EXPORTS = {
                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b200_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                  C.c_int, C.c_void_p]),
-    "b200_set_attention_impl": (C.c_int, [C.c_int]),
     "b200_ln_modulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int,
                                    C.c_int, C.c_int, C.c_void_p]),
     "b200_t2v_workspace_bytes": (C.c_size_t, [C.POINTER(T2VShape), C.c_int, C.c_int]),
@@ -160,19 +159,15 @@ EXPORTS = {
                                      C.POINTER(C.c_int), C.POINTER(C.c_int32), C.c_int]),
     # training-step passes (csrc/train.cu)
     "b200_wgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
-    "b200_dgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b200_dgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b200_linear_gelu_both": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
     "b200_transpose16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
-    "b200_cast_transpose": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b200_multi_cast": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p]),
     "b200_multi_tensor": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_cast16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b200_gate_residual": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                      C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "b200_gate_residual_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
-                                        C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "b200_gelu": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b200_gelu_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b200_gate_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int64,
                                 C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -559,8 +559,6 @@ B200_API int b200_profile_collect(double* ms_per_class, int* launches_per_class,
   return B200_OK;
 }
 
-B200_API int b200_set_attention_impl(int impl) { return b200::set_attention_impl(impl); }
-
 B200_API const char* b200_last_error(void) { return b200::get_error(); }
 B200_API int b200_abi_version(void) { return B200_ABI_VERSION; }
 
@@ -681,13 +679,12 @@ B200_API int b200_wgrad(const void* dy16, const void* x16, const float* col_scal
   a.sk_flags = static_cast<unsigned long long*>(sk_flags);
   return b200::launch_gemm(a, static_cast<cudaStream_t>(stream));
 }
-B200_API int b200_dgrad(const void* dy16, const void* w16, const void* gelu_u16, void* dx16, int rows, int n_out, int n_in, int dtype,
-                        void* stream) {
+B200_API int b200_dgrad(const void* dy16, const void* w16, void* dx16, int rows, int n_out, int n_in, int dtype, void* stream) {
   B200_DT(dtype);
   b200::GemmArgs a{};
   a.A = dy16; a.W = w16; a.M = rows; a.N = n_in; a.K = n_out; a.bf16 = dtype == B200_BF16;
-  a.epilogue = gelu_u16 ? B200_EPI_MUL_GELUGRAD16 : B200_EPI_BIAS;
-  a.add16 = gelu_u16; a.out16 = dx16; a.mn_major = 2;
+  a.epilogue = B200_EPI_BIAS;
+  a.out16 = dx16; a.mn_major = 2;
   return b200::launch_gemm(a, static_cast<cudaStream_t>(stream));
 }
 B200_API int b200_linear_gelu_both(const void* A, const void* W, const float* bias, int M, int N, int K, int dtype, void* u16, void* a16,
@@ -700,10 +697,6 @@ B200_API int b200_linear_gelu_both(const void* A, const void* W, const float* bi
 }
 B200_API int b200_transpose16(const void* in16, void* out16, int rows, int cols, void* stream) {
   return b200::launch_transpose16(in16, out16, rows, cols, static_cast<cudaStream_t>(stream));
-}
-B200_API int b200_cast_transpose(const float* in, void* out16, void* out16_t, int rows, int cols, int dtype, void* stream) {
-  B200_DT(dtype);
-  return b200::launch_cast_transpose(in, out16, out16_t, rows, cols, dtype == B200_BF16, static_cast<cudaStream_t>(stream));
 }
 B200_API int b200_multi_cast(const void* table, int n_entries, int64_t total_chunks, int dtype, void* stream) {
   B200_DT(dtype);
@@ -723,17 +716,6 @@ B200_API int b200_gate_residual(const float* x, const void* m16, const float* ga
   B200_DT(dtype);
   return b200::launch_gate_residual(x, m16, gate, gate_batch_stride, rows_per_batch, row_add, tokens, frames, out, rows, dim,
                                     dtype == B200_BF16, static_cast<cudaStream_t>(stream));
-}
-B200_API int b200_gate_residual_ln(const float* x, const void* m16, const float* gate, int64_t gate_batch_stride, const float* shift,
-                                   const float* scale, int64_t mod_batch_stride, int rows_per_batch, const float* row_add, int tokens, int frames,
-                                   float* x_out, void* h16, int rows, int dim, int dtype, void* stream) {
-  B200_DT(dtype);
-  return b200::launch_gate_residual_ln(x, m16, gate, gate_batch_stride, shift, scale, mod_batch_stride, rows_per_batch, row_add, tokens, frames,
-                                       x_out, h16, rows, dim, dtype == B200_BF16, static_cast<cudaStream_t>(stream));
-}
-B200_API int b200_gelu(const void* u16, void* a16, int64_t n, int dtype, void* stream) {
-  B200_DT(dtype);
-  return b200::launch_gelu_fwd(u16, a16, n, dtype == B200_BF16, static_cast<cudaStream_t>(stream));
 }
 B200_API int b200_gelu_bwd(const void* da16, const void* u16, void* du16, float* dbias, int rows, int dim, int dtype, void* stream) {
   B200_DT(dtype);

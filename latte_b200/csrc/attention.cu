@@ -391,13 +391,6 @@ int launch_any(int mode, int bf16, bool tail, const CUtensorMap* m, const AttnDe
 
 }  // namespace
 
-int set_attention_impl(int impl) {
-  // The Hopper build has one attention forward kernel; the switch keeps its C ABI (0 = default, 2 and 3 = the kernel
-  // generations of earlier builds) and every accepted value selects that kernel.
-  B200_REQUIRE(impl == 0 || impl == 2 || impl == 3, B200_ERR_UNSUPPORTED, "attention implementation %d unknown (0 default, 2, 3)", impl);
-  return B200_OK;
-}
-
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   B200_REQUIRE(a.batch > 0 && a.frames > 0 && a.tokens > 0 && a.heads > 0, B200_ERR_SHAPE, "attention: bad shape");
   B200_REQUIRE(a.head_dim == 64 || a.head_dim == 72 || a.head_dim == 80, B200_ERR_UNSUPPORTED,

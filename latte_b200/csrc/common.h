@@ -65,7 +65,6 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 
 // ---- device-property cache ----------------------------------------------------------------------
 int current_device(int* out);   // ordinal in [0, 64)
-int env_int(const char* name, int dflt);   // call through a function-local `static const` so the environment is read once
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per DEVICE: remember it per (kernel instantiation, device ordinal)
 struct PerDeviceOnce {
   bool done[64] = {};
@@ -105,7 +104,7 @@ struct GemmArgs {
                         // 2 = dgrad (dX[M, N] = dY[M, K] W[K, N] with the weight in its nn.Linear [out, in] layout);
                         // 1 is rejected (no caller transposes A alone)
   unsigned long long* sk_flags;  // B200_GEMM_SK_FLAGS zeroed u64 (caller's workspace) or nullptr: enables ordered stream-K
-  const void* add16;    // EPI_BIAS_ADD16: [M, N] 16-bit tensor added to the result (resnet shortcut); EPI_BIAS_MUL16 / EPI_MUL_GELUGRAD16: the factor
+  const void* add16;    // EPI_BIAS_ADD16: [M, N] 16-bit tensor added to the result (resnet shortcut); EPI_BIAS_MUL16: the factor
   void* out16b;         // EPI_BIAS_GELU_BOTH: [M, N] 16-bit second output = gelu_tanh(out16)
   // implicit-GEMM convolution (conv_taps > 0): A is an NHWC activation [conv_n, conv_h, conv_w, conv_c] (16-bit), M =
   // conv_n*conv_h*conv_w output pixels, K = conv_taps * conv_c with W laid out [N][tap][c]; tap t reads the input pixel
@@ -141,7 +140,6 @@ struct CrossAttnArgs {
   int kv_batch_rows;      // rows of the K/V buffer per sample; 0 = kv_len (T5: sequences padded to 128 rows, kv_len valid)
 };
 int launch_cross_attention(const CrossAttnArgs& a, cudaStream_t stream);
-int set_attention_impl(int impl);
 
 int launch_ln_modulate(const float* x, const float* shift, const float* scale, long long mod_batch_stride,
                        int rows_per_batch, void* out16, int rows, int dim, int bf16, cudaStream_t stream);
@@ -173,13 +171,8 @@ int launch_transpose16(const void* in, void* out, int rows, int cols, cudaStream
 int launch_multi_cast(const void* table, int n_entries, long long total_chunks, int bf16, cudaStream_t stream);
 int launch_multi_tensor(const void* table, int n_entries, long long total_chunks, int op, float a, float b, const float* scalar,
                         double* accum, cudaStream_t stream);
-int launch_cast_transpose(const float* in, void* out16, void* out16_t, int rows, int cols, int bf16, cudaStream_t stream);
 int launch_gate_residual(const float* x, const void* m16, const float* gate, long long gate_bs, int rows_per_batch,
                          const float* row_add, int tokens, int frames, float* out, int rows, int dim, int bf16, cudaStream_t stream);
-int launch_gate_residual_ln(const float* x, const void* m16, const float* gate, long long gate_bs, const float* shift, const float* scale,
-                            long long mod_bs, int rows_per_batch, const float* row_add, int tokens, int frames, float* x_out, void* h16,
-                            int rows, int dim, int bf16, cudaStream_t stream);
-int launch_gelu_fwd(const void* u16, void* a16, long long n, int bf16, cudaStream_t stream);
 int launch_gelu_bwd(const void* da16, const void* u16, void* du16, float* dbias, int rows, int dim, int bf16, cudaStream_t stream);
 int launch_gate_bwd(const float* dx, const void* m16, const float* gate, long long gate_bs, int rows_per_batch, void* dm16,
                     float* dgate, long long dgate_bs, float* dbias, int rows, int dim, int bf16, cudaStream_t stream);

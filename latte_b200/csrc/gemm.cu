@@ -149,16 +149,6 @@ struct TileSched {
   }
 };
 
-// d/dx of the tanh-form GELU with the same one-MUFU tanh
-__device__ __forceinline__ float gelu_tanh_grad(float x) {
-  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-  const float x2 = x * x;
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(k0 * fmaf(k1 * x2, x, x)));
-  const float sech2 = fmaf(-t, t, 1.0f);
-  return fmaf(0.5f * x * sech2, k0 * fmaf(3.0f * k1, x2, 1.0f), fmaf(0.5f, t, 0.5f));
-}
-
 // the residual epilogue's increment gate * (acc + bias) (+ row_add), added to x by the caller; rounded step by step (no FMA
 // contraction) so that every path through the epilogue produces the same bits
 __device__ __forceinline__ float resid_delta(float acc, float b, float gt, float ra, bool has_ra) {
@@ -410,7 +400,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 if (p.bias) { f0 += b2.x; f1 += b2.y; }
                 if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
                 uint32_t val = pack2<BF16>(f0, f1);
-                if constexpr (EPI == B200_EPI_BIAS_ADD16 || EPI == B200_EPI_BIAS_MUL16 || EPI == B200_EPI_MUL_GELUGRAD16) {
+                if constexpr (EPI == B200_EPI_BIAS_ADD16 || EPI == B200_EPI_BIAS_MUL16) {
                   const int row = m0w + lr0 + 8 * h;
                   const uint32_t side = (row < p.M && col_ok)
                       ? __ldg(reinterpret_cast<const uint32_t*>(p.add16) + (static_cast<size_t>(row) * p.N + col) / 2) : 0u;
@@ -419,8 +409,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                   if constexpr (EPI == B200_EPI_BIAS_ADD16) val = pack2<BF16>(a.x + r.x, a.y + r.y);
                   // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
                   if constexpr (EPI == B200_EPI_BIAS_MUL16) val = pack2<BF16>(a.x * r.x, a.y * r.y);
-                  // training, dgrad of fc2: du = da * gelu'(u), u (fc1's pre-activation) read back in 16 bits
-                  if constexpr (EPI == B200_EPI_MUL_GELUGRAD16) val = pack2<BF16>(a.x * gelu_tanh_grad(r.x), a.y * gelu_tanh_grad(r.y));
                 }
                 if constexpr (TWO) {           // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
                   const float2 a = unpack2<BF16>(val);
@@ -469,8 +457,8 @@ int launch_one(const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t stre
 }
 
 // Only the (epilogue, operand layout) pairs that callers launch are instantiated: every epilogue with K-major operands,
-// dgrad's bias / GELU-gradient with W stored [K, N], and wgrad's unit-gate accumulation with both operands transposed
-// (transposed operands take 128- or 256-wide tiles only).
+// dgrad's bias with W stored [K, N], and wgrad's unit-gate accumulation with both operands transposed (transposed
+// operands take 128- or 256-wide tiles only).
 template <int BN, bool BF16>
 int launch_epi(int epi, int mn, const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t s) {
   if (mn == 0) {
@@ -481,12 +469,10 @@ int launch_epi(int epi, int mn, const GemmMaps& tm, const GemmDev& p, int grid, 
       case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16, 0>(tm, p, grid, s);
       case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16, 0>(tm, p, grid, s);
       case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16, 0>(tm, p, grid, s);
-      case B200_EPI_MUL_GELUGRAD16: return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 0>(tm, p, grid, s);
     }
   }
   if constexpr (BN != 192) {
     if (mn == 2 && epi == B200_EPI_BIAS) return launch_one<BN, B200_EPI_BIAS, BF16, 2>(tm, p, grid, s);
-    if (mn == 2 && epi == B200_EPI_MUL_GELUGRAD16) return launch_one<BN, B200_EPI_MUL_GELUGRAD16, BF16, 2>(tm, p, grid, s);
     if (mn == 3 && epi == B200_EPI_GATE_RESIDUAL) return launch_one<BN, B200_EPI_GATE_RESIDUAL, BF16, 3>(tm, p, grid, s);
   }
   set_error("gemm: epilogue %d with operand layout %d and block_n %d is not built", epi, mn, BN);
@@ -501,12 +487,6 @@ int launch_bn(int bf16, int epi, int mn, const GemmMaps& tm, const GemmDev& p, i
 constexpr int kStreamKMinKb = 32;          // K / 64 below which the split costs more than the idle tail it removes
 constexpr int kSkFlags = B200_GEMM_SK_FLAGS;   // flags (u64) in the caller's buffer: 4 per streamed tile
 
-int streamk_min_kb() {
-  static const int v = env_int("B200_GEMM_SK_MINKB", kStreamKMinKb);
-  return v;
-}
-
-
 int pick_block_n(int M, int N, int K, bool resid, int sms) {
   // minimise waves x per-tile time.  A tile's cost is modelled by the operand bytes a CTA receives per k-block, A plus
   // its multicast half of W: 128 + BN/2.
@@ -516,8 +496,7 @@ int pick_block_n(int M, int N, int K, bool resid, int sms) {
   // but keeps 256 on 148 (QKV at 256 / 192: 7 / 9 waves on 132 SMs, 7 / 8 on 148), and the 148-SM choices are kept as
   // tests/test_schedule.py states them, so the rule is unchanged.
   if (N <= 128) return 128;   // narrow outputs (e.g. the VAE's 3-channel conv_out padded to 32): smallest tile that covers N
-  static const bool no_sk = env_int("B200_GEMM_NO_STREAMK", 0) != 0;
-  const bool sk = resid && !no_sk && K / BK >= streamk_min_kb();
+  const bool sk = resid && K / BK >= kStreamKMinKb;
   const int cand[3] = {256, 192, 128};
   int best = 128;
   double best_cost = 1e300;
@@ -533,7 +512,6 @@ int pick_block_n(int M, int N, int K, bool resid, int sms) {
 // The scheduling decisions of one launch (shared by launch_gemm and the schedule dump the CPU tests read).
 struct GemmPlan { int bn, pairs, pair_tiles, num_kb, streamk; };
 GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool split_small = false) {
-  static const bool no_sk = env_int("B200_GEMM_NO_STREAMK", 0) != 0;
   GemmPlan g;
   g.bn = block_n ? block_n : pick_block_n(M, N, K, resid, sms);
   const int num_m = (M + BM - 1) / BM, num_n = (N + g.bn - 1) / g.bn;
@@ -541,12 +519,12 @@ GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool s
   const int grid = 2 * g.pair_tiles < sms ? 2 * g.pair_tiles : (sms & ~1);   // whole clusters of 2
   g.pairs = grid / 2;
   g.num_kb = K / BK;
-  g.streamk = (resid && !no_sk && g.pair_tiles > g.pairs && g.pair_tiles % g.pairs != 0 && g.num_kb >= streamk_min_kb()) ? 1 : 0;
+  g.streamk = (resid && g.pair_tiles > g.pairs && g.pair_tiles % g.pairs != 0 && g.num_kb >= kStreamKMinKb) ? 1 : 0;
   // weight gradients: a small output (fewer tiles than CTA pairs) under a very long contraction (K = tokens).  All tiles are
   // streamed: the (tile, k-block) units are cut into one equal share per pair, a tile's partial sums are reduce-added in k
   // order through the same flags (a chain of waits only ever points from pair p+1 to pair p, and every pair is resident).
-  if (split_small && resid && !no_sk && g.pair_tiles <= sms / 2 && g.pair_tiles % (sms / 2) != 0 &&
-      static_cast<long long>(g.pair_tiles) * g.num_kb >= static_cast<long long>(sms / 2) * streamk_min_kb()) {
+  if (split_small && resid && g.pair_tiles <= sms / 2 && g.pair_tiles % (sms / 2) != 0 &&
+      static_cast<long long>(g.pair_tiles) * g.num_kb >= static_cast<long long>(sms / 2) * kStreamKMinKb) {
     g.pairs = sms / 2;
     g.streamk = 1;
   }
@@ -587,14 +565,13 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   B200_REQUIRE(a.K % BK == 0, B200_ERR_SHAPE, "gemm: K=%d must be a multiple of %d", a.K, BK);
   B200_REQUIRE(a.N % 32 == 0, B200_ERR_SHAPE, "gemm: N=%d must be a multiple of 32", a.N);
   B200_REQUIRE(a.epilogue == B200_EPI_BIAS || a.epilogue == B200_EPI_BIAS_GELU || a.epilogue == B200_EPI_GATE_RESIDUAL ||
-                   a.epilogue == B200_EPI_BIAS_ADD16 || a.epilogue == B200_EPI_BIAS_MUL16 || a.epilogue == B200_EPI_BIAS_GELU_BOTH ||
-                   a.epilogue == B200_EPI_MUL_GELUGRAD16,
+                   a.epilogue == B200_EPI_BIAS_ADD16 || a.epilogue == B200_EPI_BIAS_MUL16 || a.epilogue == B200_EPI_BIAS_GELU_BOTH,
                B200_ERR_UNSUPPORTED, "gemm: unknown epilogue %d", a.epilogue);
-  B200_REQUIRE((a.epilogue != B200_EPI_BIAS_ADD16 && a.epilogue != B200_EPI_BIAS_MUL16 && a.epilogue != B200_EPI_MUL_GELUGRAD16) ||
+  B200_REQUIRE((a.epilogue != B200_EPI_BIAS_ADD16 && a.epilogue != B200_EPI_BIAS_MUL16) ||
                    (a.add16 && (reinterpret_cast<uintptr_t>(a.add16) & 15) == 0), B200_ERR_ALIGN, "gemm: add16 tensor missing or unaligned");
   B200_REQUIRE(a.epilogue != B200_EPI_BIAS_GELU_BOTH || (a.out16b && (reinterpret_cast<uintptr_t>(a.out16b) & 15) == 0), B200_ERR_ALIGN,
                "gemm: second output missing or unaligned");
-  B200_REQUIRE((a.epilogue != B200_EPI_BIAS_GELU_BOTH && a.epilogue != B200_EPI_MUL_GELUGRAD16) || a.N % 8 == 0, B200_ERR_SHAPE, "gemm: N %% 8");
+  B200_REQUIRE(a.epilogue != B200_EPI_BIAS_GELU_BOTH || a.N % 8 == 0, B200_ERR_SHAPE, "gemm: N %% 8");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(a.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.W) & 15) == 0,
                B200_ERR_ALIGN, "gemm: A and W must be 16-byte aligned");
   const bool resid = a.epilogue == B200_EPI_GATE_RESIDUAL;
@@ -624,9 +601,8 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
       block_n = pick_block_n(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, sms);
       if (block_n == 192) block_n = (a.N % 256 == 0 || a.N > 1024) ? 256 : 128;     // W chunks are 64 wide per CTA: 128 or 256 only
       // weight gradients: 256-wide tiles for every output of at least 256 columns (the tiles are split along K anyway, so
-      // the wider tile only halves the A traffic); B200_WGRAD_BN=128|256 forces a width for A/B runs
-      static const int wgrad_bn = env_int("B200_WGRAD_BN", 0);
-      if (a.mn_major == 3) block_n = (wgrad_bn == 128 || wgrad_bn == 256) ? wgrad_bn : (a.N >= 256 ? 256 : block_n);
+      // the wider tile only halves the A traffic)
+      if (a.mn_major == 3) block_n = a.N >= 256 ? 256 : block_n;
     }
   }
   const GemmPlan plan = plan_gemm(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, a.mn_major == 3);
@@ -712,7 +688,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   const int grid = 2 * plan.pairs;
   {
     // stream-K over the last waves: only where partial sums can be reduce-added (residual epilogue) and K is long enough
-    // to be worth splitting (plan_gemm); B200_GEMM_NO_STREAMK=1 restores the one-add-per-element schedule.
+    // to be worth splitting (plan_gemm).
     const int pairs = plan.pairs;
     // the ordering flags live in the CALLER's buffer (zeroed once; every launch leaves it zeroed): without one the
     // schedule stays data-parallel

@@ -129,12 +129,6 @@ int encode_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, co
 }
 }  // namespace
 
-// ---- experiment switches: read from the environment ONCE per process (they select code paths for A/B timing only)
-int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
 namespace {
 struct DevInfo {
   int valid = 0, major = 0, minor = 0, sms = 0;

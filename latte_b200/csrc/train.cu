@@ -1,13 +1,16 @@
 // Backward-pass kernels of the training step (BASELINE config 5; reference train.py:206-222 -> autograd over models/latte.py).
 // Every GEMM of the backward (dgrad, wgrad) runs on the wgmma kernel of gemm.cu; this file holds what surrounds them:
-//   transpose16 / cast_transpose   16-bit [R,C] -> [C,R] operands for wgrad (K = tokens must be the contiguous dimension)
+//   transpose16                    16-bit [R,C] -> [C,R] operands for wgrad (K = tokens must be the contiguous dimension)
+//   multi_cast / multi_tensor      fp32 -> 16-bit operand copies; gradient norm, clipping and EMA, many tensors per launch
 //   gate_residual                  x_out = x + gate[b] * m (+ temp_embed row)          forward of latte.py:179-180 residuals
-//   gelu_fwd / gelu_bwd            tanh-GELU and its derivative, bias gradient (column sums) fused      (latte.py:169-171)
+//   gelu_bwd                       tanh-GELU derivative, bias gradient (column sums) fused               (latte.py:169-171)
 //   gate_bwd                       dm = dx * gate[b]; dgate[b] = sum_rows dx * m; dbias = sum_rows dm   (latte.py:179-180)
+//   colsum                         column sums (bias gradients of the plain Linear layers)
 //   ln_modulate_bwd                d/dx of LN(x)(1+scale)+shift accumulated into dx; dshift, dscale per sample (latte.py:28-29)
 //   attn_bwd_dq / attn_bwd_dkv     softmax(QK^T hd^-1/2)V backward on mma.sync tensor cores, scores recomputed (latte.py:48-77)
 //                                  (also the temporal sequences of 17..128 frames: strided rows, partial last block masked)
-//   attn_bwd_temporal(_mma)        same for the F <= 16 frame sequences (one 16-row tile per (b, n, head))
+//   attn_bwd_temporal_mma          same for the F <= 16 frame sequences (one 16-row tile per (b, n, head))
+// The attention backward takes head_dim 64 or 72 only.
 //   ada_outer / ada_dsc            gradients of the stacked adaLN_modulation Linear on B rows  (latte.py:160-163,192-195)
 // All are HBM-bound passes (one read, one write, fp32 math) except the attention backward (tensor cores, ~2 % of the FLOPs).
 #include "common.h"
@@ -53,67 +56,6 @@ __global__ void __launch_bounds__(256) transpose16_kernel(const uint16_t* __rest
     if (orow < C && ocol < R) {
       const uint32_t v = static_cast<uint32_t>(tile[2 * tx][c]) | (static_cast<uint32_t>(tile[2 * tx + 1][c]) << 16);
       *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(orow) * R + ocol) = v;
-    }
-  }
-}
-
-// fp32 [R,C] -> 16-bit [R,C] and 16-bit [C,R] in one read (weights: W for the forward GEMM, W^T as the dgrad weight operand)
-template <bool BF16>
-__global__ void __launch_bounds__(256) cast_transpose_kernel(const float* __restrict__ in, uint16_t* __restrict__ out,
-                                                             uint16_t* __restrict__ out_t, int R, int C) {
-  __shared__ uint16_t tile[64][66];
-  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (int r = ty; r < 64; r += 8) {
-    const int row = r0 + r, col = c0 + 2 * tx;
-    uint32_t v = 0;
-    if (row < R && col < C) {
-      const float2 f = *reinterpret_cast<const float2*>(in + static_cast<size_t>(row) * C + col);
-      v = pack2<BF16>(f.x, f.y);
-      *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row) * C + col) = v;
-    }
-    tile[r][2 * tx] = static_cast<uint16_t>(v & 0xffffu);
-    tile[r][2 * tx + 1] = static_cast<uint16_t>(v >> 16);
-  }
-  if (out_t == nullptr) return;
-  __syncthreads();
-  for (int c = ty; c < 64; c += 8) {
-    const int orow = c0 + c, ocol = r0 + 2 * tx;
-    if (orow < C && ocol < R) {
-      const uint32_t v = static_cast<uint32_t>(tile[2 * tx][c]) | (static_cast<uint32_t>(tile[2 * tx + 1][c]) << 16);
-      *reinterpret_cast<uint32_t*>(out_t + static_cast<size_t>(orow) * R + ocol) = v;
-    }
-  }
-}
-
-// wide version for R % 4 == 0 and C % 4 == 0 (every weight matrix): 16-byte reads, 8-byte writes on both outputs
-template <bool BF16>
-__global__ void __launch_bounds__(256) cast_transpose4_kernel(const float* __restrict__ in, uint16_t* __restrict__ out,
-                                                              uint16_t* __restrict__ out_t, int R, int C) {
-  __shared__ uint16_t tile[64][66];
-  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-#pragma unroll
-  for (int r = ty; r < 64; r += 16) {
-    const int row = r0 + r, col = c0 + 4 * tx;
-    uint2 v = make_uint2(0, 0);
-    if (row < R && col < C) {
-      const float4 f = *reinterpret_cast<const float4*>(in + static_cast<size_t>(row) * C + col);
-      v = make_uint2(pack2<BF16>(f.x, f.y), pack2<BF16>(f.z, f.w));
-      *reinterpret_cast<uint2*>(out + static_cast<size_t>(row) * C + col) = v;
-    }
-    *reinterpret_cast<uint32_t*>(&tile[r][4 * tx]) = v.x;
-    *reinterpret_cast<uint32_t*>(&tile[r][4 * tx + 2]) = v.y;
-  }
-  if (out_t == nullptr) return;
-  __syncthreads();
-#pragma unroll
-  for (int c = ty; c < 64; c += 16) {
-    const int orow = c0 + c, ocol = r0 + 4 * tx;
-    if (orow < C && ocol < R) {
-      const uint32_t lo = static_cast<uint32_t>(tile[4 * tx][c]) | (static_cast<uint32_t>(tile[4 * tx + 1][c]) << 16);
-      const uint32_t hi = static_cast<uint32_t>(tile[4 * tx + 2][c]) | (static_cast<uint32_t>(tile[4 * tx + 3][c]) << 16);
-      *reinterpret_cast<uint2*>(out_t + static_cast<size_t>(orow) * R + ocol) = make_uint2(lo, hi);
     }
   }
 }
@@ -229,72 +171,6 @@ __global__ void __launch_bounds__(256) gate_residual_kernel(const float* __restr
   }
 }
 
-// gate_residual + the LayerNorm-modulate that always follows it, in one pass: x_out = x + gate[b] * m (+ row_add), written for the
-// backward, and h = LN(x_out) * (1 + scale[b]) + shift[b] as the next GEMM's 16-bit operand -- the row never leaves registers
-// between the two (saves re-reading the 94 MB stream per pair at local batch 5).  One warp per row, rows dealt round-robin.
-template <bool BF16, int NV, int MINB>
-__global__ void __launch_bounds__(128, MINB) gate_residual_ln_kernel(const float* __restrict__ x, const uint16_t* __restrict__ m,
-                                                               const float* __restrict__ gate, long long gate_bs,
-                                                               const float* __restrict__ shift, const float* __restrict__ scale, long long mod_bs,
-                                                               int rpb, const float* __restrict__ row_add, int tokens, int frames,
-                                                               float* __restrict__ x_out, uint16_t* __restrict__ h, int rows, int dim) {
-  const int lane = threadIdx.x & 31;
-  const int nv = dim >> 2;
-  const int warps = (gridDim.x * blockDim.x) >> 5;
-  const float inv_d = 1.0f / static_cast<float>(dim);
-  for (int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
-    const int b = row / rpb;
-    const float4* xr = reinterpret_cast<const float4*>(x + static_cast<size_t>(row) * dim);
-    const uint2* mr = reinterpret_cast<const uint2*>(m + static_cast<size_t>(row) * dim);
-    const float4* g4 = reinterpret_cast<const float4*>(gate + b * gate_bs);
-    const float4* ra = row_add ? reinterpret_cast<const float4*>(row_add + static_cast<size_t>((row / tokens) % frames) * dim) : nullptr;
-    float4 v[NV];
-    uint2 mv[NV];
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int idx = lane + i * 32;
-      if (idx < nv) { v[i] = xr[idx]; mv[i] = mr[idx]; }
-    }
-    float s = 0.f;
-    float4* xo = reinterpret_cast<float4*>(x_out + static_cast<size_t>(row) * dim);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int idx = lane + i * 32;
-      if (idx < nv) {
-        const float4 g = __ldg(g4 + idx);
-        const float2 m0 = unpack2<BF16>(mv[i].x), m1 = unpack2<BF16>(mv[i].y);
-        v[i].x = fmaf(g.x, m0.x, v[i].x); v[i].y = fmaf(g.y, m0.y, v[i].y); v[i].z = fmaf(g.z, m1.x, v[i].z); v[i].w = fmaf(g.w, m1.y, v[i].w);
-        if (ra) { const float4 a = __ldg(ra + idx); v[i].x += a.x; v[i].y += a.y; v[i].z += a.z; v[i].w += a.w; }
-        xo[idx] = v[i];
-        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-      }
-    }
-    const float mean = warp_sum(s) * inv_d;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      if (lane + i * 32 < nv) {
-        const float a = v[i].x - mean, bb = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-        q += (a * a + bb * bb) + (c * c + d * d);
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(q) * inv_d + 1e-6f);
-    const float4* sh = reinterpret_cast<const float4*>(shift + b * mod_bs);
-    const float4* sc = reinterpret_cast<const float4*>(scale + b * mod_bs);
-    uint2* hr = reinterpret_cast<uint2*>(h + static_cast<size_t>(row) * dim);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int idx = lane + i * 32;
-      if (idx < nv) {
-        const float4 a = __ldg(sh + idx), c = __ldg(sc + idx);
-        const float y0 = fmaf((v[i].x - mean) * rstd, 1.0f + c.x, a.x), y1 = fmaf((v[i].y - mean) * rstd, 1.0f + c.y, a.y);
-        const float y2 = fmaf((v[i].z - mean) * rstd, 1.0f + c.z, a.z), y3 = fmaf((v[i].w - mean) * rstd, 1.0f + c.w, a.w);
-        hr[idx] = make_uint2(pack2<BF16>(y0, y1), pack2<BF16>(y2, y3));
-      }
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ GELU (tanh form)
 // one MUFU op per element (tanh.approx, relative error 2^-11 -- below the 16-bit rounding of the result), as in the GEMM's
 // GELU epilogue: with libm's tanhf the backward pass was ALU-bound (~60 instructions per element on 94 M elements per call)
@@ -302,11 +178,6 @@ __device__ __forceinline__ float tanh_fast(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-__device__ __forceinline__ float gelu_f(float u) {
-  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-  const float hu = 0.5f * u;
-  return fmaf(hu, tanh_fast(k0 * fmaf(k1 * u * u, u, u)), hu);
 }
 __device__ __forceinline__ float gelu_grad(float u) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
@@ -316,35 +187,17 @@ __device__ __forceinline__ float gelu_grad(float u) {
   return fmaf(0.5f * u * sech2, k0 * fmaf(3.0f * k1, u2, 1.0f), fmaf(0.5f, th, 0.5f));
 }
 
-template <bool BF16>
-__global__ void __launch_bounds__(256) gelu_fwd_kernel(const uint16_t* __restrict__ u, uint16_t* __restrict__ a, long long n8) {
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const uint4 v = reinterpret_cast<const uint4*>(u)[i];
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack2<BF16>(w[j]);
-      o[j] = pack2<BF16>(gelu_f(f.x), gelu_f(f.y));
-    }
-    reinterpret_cast<uint4*>(a)[i] = make_uint4(o[0], o[1], o[2], o[3]);
-  }
-}
-
-// du = da * gelu'(u); dbias[c] += sum over the block's rows.  Block = 128 threads x 8 columns, `rs` rows per block.
+// du = da * gelu'(u); dbias[c] += sum over the block's rows.  Block = 128 threads x 8 columns.
 template <bool BF16>
 __global__ void __launch_bounds__(128) gelu_bwd_kernel(const uint16_t* __restrict__ da, const uint16_t* __restrict__ u,
-                                                       uint16_t* __restrict__ du, float* __restrict__ dbias, int rows, int dim, int rs, int dbg) {
+                                                       uint16_t* __restrict__ du, float* __restrict__ dbias, int rows, int dim) {
   // Rows are dealt round-robin to the gridDim.y row-lanes (lane y takes rows y, y + G, ...): at any moment the whole grid
-  // works inside one sliding window of G consecutive rows, which DRAM serves far better than G far-apart row slabs
-  // (measured: 165 -> see profiles/r02_train_micro.txt).  `rs` = rows per lane.
+  // works inside one sliding window of G consecutive rows, which DRAM serves far better than G far-apart row slabs.
   const int c8 = blockIdx.x * 128 + threadIdx.x;
   if (c8 * 8 >= dim) return;
   const int G = gridDim.y;
   float acc[8] = {};
   const int nv = dim >> 3;
-  (void)rs;
   // explicit load batches: U rows of both streams are requested before any of them is consumed (left to itself the compiler
   // interleaves load -> math -> store per row and keeps ~2 rows in flight per thread)
   constexpr int U = 4;
@@ -377,19 +230,17 @@ __global__ void __launch_bounds__(128) gelu_bwd_kernel(const uint16_t* __restric
       }
     }
   }
-  if (dbg & 1) return;
 #pragma unroll
   for (int j = 0; j < 8; ++j) atomicAdd(dbias + c8 * 8 + j, acc[j]);
 }
 
 // ------------------------------------------------------------------------------------------------ gate_bwd
-// dm = dx * gate[b] (16-bit); dgate[b, c] += sum_rows dx * m; dbias[c] += sum_rows dm.  Thread = 4 columns, `rs` rows/block
-// (rs divides rows_per_batch, so a block stays inside one sample).
+// dm = dx * gate[b] (16-bit); dgate[b, c] += sum_rows dx * m; dbias[c] += sum_rows dm.  Thread = 4 columns.
 template <bool BF16>
 __global__ void __launch_bounds__(128) gate_bwd_kernel(const float* __restrict__ dx, const uint16_t* __restrict__ m,
                                                        const float* __restrict__ gate, long long gate_bs, int rpb,
                                                        uint16_t* __restrict__ dm, float* __restrict__ dgate, long long dgate_bs,
-                                                       float* __restrict__ dbias, int rows, int dim, int rs, int dbg) {
+                                                       float* __restrict__ dbias, int rows, int dim) {
   // grid (column strips, G row-lanes, samples): lane y of sample b takes rows b*rpb + y, + G, ... (sliding window, see gelu_bwd)
   const int c4 = blockIdx.x * 128 + threadIdx.x;
   const int nv = dim >> 2;
@@ -398,7 +249,6 @@ __global__ void __launch_bounds__(128) gate_bwd_kernel(const float* __restrict__
   const int b = blockIdx.z;
   const int r0 = b * rpb + blockIdx.y;
   const int r1 = min(rows, (b + 1) * rpb);
-  (void)rs;
   const float4 g = __ldg(reinterpret_cast<const float4*>(gate + b * gate_bs) + c4);
   float ag[4] = {}, ab[4] = {};
   constexpr int U = 8;            // explicit load batches, see gelu_bwd
@@ -427,7 +277,6 @@ __global__ void __launch_bounds__(128) gate_bwd_kernel(const float* __restrict__
       }
     }
   }
-  if (dbg & 1) return;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     atomicAdd(dgate + b * dgate_bs + c4 * 4 + j, ag[j]);
@@ -437,12 +286,11 @@ __global__ void __launch_bounds__(128) gate_bwd_kernel(const float* __restrict__
 
 // column sums of a [rows, dim] matrix (16-bit or fp32) into fp32 (pre-zeroed)
 template <int KIND>   // 0 fp32, 1 fp16, 2 bf16
-__global__ void __launch_bounds__(128) colsum_kernel(const void* __restrict__ a, float* __restrict__ out, int rows, int dim, int rs) {
+__global__ void __launch_bounds__(128) colsum_kernel(const void* __restrict__ a, float* __restrict__ out, int rows, int dim) {
   const int c4 = blockIdx.x * 128 + threadIdx.x;
   const int nv = dim >> 2;
   if (c4 >= nv) return;
   const int G = gridDim.y;
-  (void)rs;
   float acc[4] = {};
   constexpr int U = 8;            // explicit load batches, see gelu_bwd
   for (int r = blockIdx.y; r < rows; r += U * G) {
@@ -475,15 +323,14 @@ __global__ void __launch_bounds__(128) colsum_kernel(const void* __restrict__ a,
 // h = xhat * (1 + scale[b]) + shift[b], xhat = (x - mean) * rstd.  Given dh:
 //   dshift[b] += sum_rows dh;  dscale[b] += sum_rows dh * xhat;  g = dh * (1 + scale[b]);
 //   dx += rstd * (g - mean(g) - xhat * mean(g * xhat)).
-// One warp per row (row in registers), LB_RPW consecutive rows per warp, the 4 warps of a block reduce their column sums
-// through shared memory before the atomics.  rows_per_batch % (4 * LB_RPW) == 0 keeps a block inside one sample.
+// One warp per row (row in registers); the warps of a block reduce their column sums through shared memory before the
+// atomics.
 
 template <bool BF16, int NV>
 __global__ void __launch_bounds__(256) ln_modulate_bwd_kernel(const uint16_t* __restrict__ dh, const float* __restrict__ x,
                                                               const float* __restrict__ scale, long long mod_bs, int rpb,
                                                               float* __restrict__ dx, float* __restrict__ dshift,
-                                                              float* __restrict__ dscale, long long dmod_bs, int rows, int dim,
-                                                              int rpw, int dbg) {
+                                                              float* __restrict__ dscale, long long dmod_bs, int rows, int dim) {
   extern __shared__ float s_red[];   // [warps][2][dim]: per-warp column sums of dh and dh * xhat (each lane owns its columns)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nw = blockDim.x >> 5;
@@ -502,7 +349,6 @@ __global__ void __launch_bounds__(256) ln_modulate_bwd_kernel(const uint16_t* __
     if (idx < nv) red_sh[idx] = red_sc[idx] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   const float inv_d = 1.0f / static_cast<float>(dim);
-  (void)rpw;
   for (int rr = gw; rr < rpb; rr += W) {
     const int row = b * rpb + rr;
     if (row >= rows) break;
@@ -570,7 +416,6 @@ __global__ void __launch_bounds__(256) ln_modulate_bwd_kernel(const uint16_t* __
     }
   }
   __syncthreads();
-  if (dbg & 1) return;
   for (int i = threadIdx.x; i < 2 * dim; i += blockDim.x) {
     const int which = i / dim, c = i % dim;
     float t = 0.f;
@@ -982,84 +827,9 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const uint16_t* __res
 }
 
 // ------------------------------------------------------------------------------------------------ attention backward (temporal)
-// Sequences of F <= 16 frames at a fixed token: rows (b, f, n), f = 0..F-1 (row stride `tokens`).  One CTA of 128 threads per
-// (b, n, head); everything lives in shared memory as fp32.  HBM-bound (reads qkv + dO, writes dqkv).
-template <bool BF16>
-__global__ void __launch_bounds__(128) attn_bwd_temporal_kernel(const uint16_t* __restrict__ qkv, const uint16_t* __restrict__ d_o,
-                                                                uint16_t* __restrict__ dqkv, int frames, int tokens, int heads,
-                                                                int hd, float scale) {
-  extern __shared__ float sf[];
-  const int F = frames;
-  const int hdp = hd + 1;        // odd pitch: the F x F score loop reads rows of q/k/v/g at stride hdp -> conflict-free
-  float* q = sf;                 // [F][hdp]
-  float* k = q + F * hdp;
-  float* v = k + F * hdp;
-  float* g = v + F * hdp;        // dO
-  float* P = g + F * hdp;        // [F][F]
-  float* dS = P + F * F;         // [F][F]
-  const int n = blockIdx.x % tokens, b = blockIdx.x / tokens, h = blockIdx.y;
-  const int D = heads * hd, ld = 3 * D;
-  const size_t row0 = static_cast<size_t>(b) * F * tokens + n;
-  const int c8n = hd / 8;        // 16-byte chunks per row
-  for (int i = threadIdx.x; i < 4 * F * c8n; i += blockDim.x) {
-    const int which = i / (F * c8n), rem = i % (F * c8n);
-    const int f = rem / c8n, c = (rem % c8n) * 8;
-    const size_t r = row0 + static_cast<size_t>(f) * tokens;
-    const uint16_t* src = which < 3 ? qkv + r * ld + which * D + h * hd + c : d_o + r * D + h * hd + c;
-    const uint4 u = *reinterpret_cast<const uint4*>(src);
-    float* dst = sf + which * F * hdp + f * hdp + c;
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 t = unpack2<BF16>(w[j]);
-      dst[2 * j] = t.x;
-      dst[2 * j + 1] = t.y;
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < F * F; i += blockDim.x) {
-    const int a = i / F, c = i % F;
-    float sacc = 0.f, dp = 0.f;
-    for (int d = 0; d < hd; ++d) {
-      sacc += q[a * hdp + d] * k[c * hdp + d];
-      dp += g[a * hdp + d] * v[c * hdp + d];
-    }
-    P[i] = sacc * scale;
-    dS[i] = dp;
-  }
-  __syncthreads();
-  if (threadIdx.x < F) {
-    const int a = threadIdx.x;
-    float m = -INFINITY;
-    for (int c = 0; c < F; ++c) m = fmaxf(m, P[a * F + c]);
-    float t = 0.f;
-    for (int c = 0; c < F; ++c) { const float e = __expf(P[a * F + c] - m); P[a * F + c] = e; t += e; }
-    const float inv = 1.0f / t;
-    float dl = 0.f;
-    for (int c = 0; c < F; ++c) { P[a * F + c] *= inv; dl += P[a * F + c] * dS[a * F + c]; }
-    for (int c = 0; c < F; ++c) dS[a * F + c] = P[a * F + c] * (dS[a * F + c] - dl) * scale;
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 3 * F * c8n; i += blockDim.x) {
-    const int which = i / (F * c8n), rem = i % (F * c8n);
-    const int f = rem / c8n, c = (rem % c8n) * 8;
-    float acc[8] = {};
-    for (int j = 0; j < F; ++j) {
-      // dq_f = sum_j dS[f][j] k_j;  dk_f = sum_j dS[j][f] q_j;  dv_f = sum_j P[j][f] dO_j
-      const float wgt = which == 0 ? dS[f * F + j] : (which == 1 ? dS[j * F + f] : P[j * F + f]);
-      const float* src = (which == 0 ? k : (which == 1 ? q : g)) + j * hdp + c;
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] = fmaf(wgt, src[e], acc[e]);
-    }
-    const size_t r = row0 + static_cast<size_t>(f) * tokens;
-    *reinterpret_cast<uint4*>(dqkv + r * ld + which * D + h * hd + c) =
-        make_uint4(pack2<BF16>(acc[0], acc[1]), pack2<BF16>(acc[2], acc[3]), pack2<BF16>(acc[4], acc[5]), pack2<BF16>(acc[6], acc[7]));
-  }
-}
-
-// Tensor-core version of the above for head_dim 64 / 72: ONE WARP per (b, n, head), four heads per CTA, no block-level
-// synchronisation.  The F <= 16 frames of q, k, v, dO sit in a [16 x HDP] shared tile each (rows >= F zero); S = Q K^T and
-// dP = dO V^T are one 16x16 accumulator pair, and the transposed pair (K Q^T, V dO^T) is recomputed so that P^T / dS^T come
+// Sequences of F <= 16 frames at a fixed token: rows (b, f, n), f = 0..F-1 (row stride `tokens`), head_dim 64 / 72, on tensor
+// cores.  ONE WARP per (b, n, head), four heads per CTA, no block-level synchronisation.  The F <= 16 frames of q, k, v, dO
+// sit in a [16 x HDP] shared tile each (rows >= F zero); S = Q K^T and dP = dO V^T are one 16x16 accumulator pair, and the transposed pair (K Q^T, V dO^T) is recomputed so that P^T / dS^T come
 // out directly as the A operands of dV = P^T dO and dK = dS^T Q (as in the spatial kernel B).  Row statistics go through 32
 // floats of shared memory.  Results are staged in the tiles they came from and written back with 16-byte stores.
 template <bool BF16, int HD>
@@ -1310,23 +1080,6 @@ int launch_transpose16(const void* in, void* out, int rows, int cols, cudaStream
   return B200_OK;
 }
 
-int launch_cast_transpose(const float* in, void* out16, void* out16_t, int rows, int cols, int bf16, cudaStream_t stream) {
-  B200_REQUIRE(rows > 0 && cols > 0 && rows % 2 == 0 && cols % 2 == 0, B200_ERR_SHAPE, "cast_transpose: %d x %d must be even", rows, cols);
-  B200_REQUIRE((reinterpret_cast<uintptr_t>(in) & 7) == 0 && (reinterpret_cast<uintptr_t>(out16) & 3) == 0 &&
-                   (reinterpret_cast<uintptr_t>(out16_t) & 3) == 0, B200_ERR_ALIGN, "cast_transpose: misaligned pointer");
-  dim3 grid((cols + 63) / 64, (rows + 63) / 64);
-  uint16_t *o = static_cast<uint16_t*>(out16), *ot = static_cast<uint16_t*>(out16_t);
-  const bool wide = rows % 4 == 0 && cols % 4 == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0 && (reinterpret_cast<uintptr_t>(o) & 7) == 0 &&
-                    (reinterpret_cast<uintptr_t>(ot) & 7) == 0;
-  if (wide) {
-    if (bf16) cast_transpose4_kernel<true><<<grid, 256, 0, stream>>>(in, o, ot, rows, cols);
-    else cast_transpose4_kernel<false><<<grid, 256, 0, stream>>>(in, o, ot, rows, cols);
-  } else if (bf16) cast_transpose_kernel<true><<<grid, 256, 0, stream>>>(in, o, ot, rows, cols);
-  else cast_transpose_kernel<false><<<grid, 256, 0, stream>>>(in, o, ot, rows, cols);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return B200_OK;
-}
-
 int launch_multi_cast(const void* table, int n_entries, long long total_chunks, int bf16, cudaStream_t stream) {
   B200_REQUIRE(table != nullptr && n_entries > 0 && total_chunks > 0, B200_ERR_SHAPE, "multi_cast: empty table");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(table) & 7) == 0, B200_ERR_ALIGN, "multi_cast: table must be 8-byte aligned");
@@ -1369,77 +1122,31 @@ int launch_gate_residual(const float* x, const void* m16, const float* gate, lon
   return B200_OK;
 }
 
-template <bool BF16, int NV>
-static int grl_launch(cudaStream_t stream, const float* x, const uint16_t* m, const float* gate, long long gate_bs, const float* shift,
-                      const float* scale, long long mod_bs, int rpb, const float* row_add, int tokens, int frames, float* x_out, uint16_t* h,
-                      int rows, int dim) {
-  static const int minb = env_int("B200_GRL_MINB", 5);     // A/B switch: register cap (5 blocks of 4 warps per SM: 96 registers) vs none (134)
-  const int blocks = rows / 4 < 132 * 8 ? (rows + 3) / 4 : 132 * 8;
-  if (minb >= 5) gate_residual_ln_kernel<BF16, NV, 5><<<blocks, 128, 0, stream>>>(x, m, gate, gate_bs, shift, scale, mod_bs, rpb, row_add, tokens, frames, x_out, h, rows, dim);
-  else gate_residual_ln_kernel<BF16, NV, 1><<<blocks, 128, 0, stream>>>(x, m, gate, gate_bs, shift, scale, mod_bs, rpb, row_add, tokens, frames, x_out, h, rows, dim);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return B200_OK;
-}
-
-int launch_gate_residual_ln(const float* x, const void* m16, const float* gate, long long gate_bs, const float* shift, const float* scale,
-                            long long mod_bs, int rows_per_batch, const float* row_add, int tokens, int frames, float* x_out, void* h16,
-                            int rows, int dim, int bf16, cudaStream_t stream) {
-  B200_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && dim <= 12 * 128 && rows_per_batch > 0 && gate_bs % 4 == 0 && mod_bs % 4 == 0, B200_ERR_SHAPE,
-               "gate_residual_ln: bad shape");
-  B200_REQUIRE(row_add == nullptr || (tokens > 0 && frames > 0), B200_ERR_SHAPE, "gate_residual_ln: row_add needs tokens and frames");
-  B200_REQUIRE(ALIGNED16(x) && ALIGNED16(gate) && ALIGNED16(shift) && ALIGNED16(scale) && ALIGNED16(x_out) && (reinterpret_cast<uintptr_t>(m16) & 7) == 0 &&
-                   (reinterpret_cast<uintptr_t>(h16) & 7) == 0 && (row_add == nullptr || ALIGNED16(row_add)), B200_ERR_ALIGN, "gate_residual_ln: misaligned pointer");
-  const uint16_t* m = static_cast<const uint16_t*>(m16);
-  uint16_t* h = static_cast<uint16_t*>(h16);
-  const int nvmax = (dim / 4 + 31) / 32;
-#define GRL(BF, NVV) return grl_launch<BF, NVV>(stream, x, m, gate, gate_bs, shift, scale, mod_bs, rows_per_batch, row_add, tokens, frames, x_out, h, rows, dim)
-  if (bf16) {
-    if (nvmax <= 3) GRL(true, 3);
-    if (nvmax <= 6) GRL(true, 6);
-    if (nvmax <= 9) GRL(true, 9);
-    GRL(true, 12);
-  }
-  if (nvmax <= 3) GRL(false, 3);
-  if (nvmax <= 6) GRL(false, 6);
-  if (nvmax <= 9) GRL(false, 9);
-  GRL(false, 12);
-#undef GRL
-}
-
-int launch_gelu_fwd(const void* u16, void* a16, long long n, int bf16, cudaStream_t stream) {
-  B200_REQUIRE(n > 0 && n % 8 == 0, B200_ERR_SHAPE, "gelu: element count %lld must be a multiple of 8", n);
-  B200_REQUIRE(ALIGNED16(u16) && ALIGNED16(a16), B200_ERR_ALIGN, "gelu: pointers must be 16-byte aligned");
-  const int blocks = grid_for(n / 8, 256, 132 * 16);
-  if (bf16) gelu_fwd_kernel<true><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(u16), static_cast<uint16_t*>(a16), n / 8);
-  else gelu_fwd_kernel<false><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(u16), static_cast<uint16_t*>(a16), n / 8);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return B200_OK;
-}
+// Row-lanes of the column-sum passes (gridDim.y = rows / rows per lane) and the warps of ln_modulate_bwd
+constexpr int kGeluBwdRowsPerLane = 32, kGateBwdRowsPerLane = 32, kColsumRowsPerLane = 64;
+constexpr int kLnbWarps = 4, kLnbRowsPerWarp = 8;
 
 int launch_gelu_bwd(const void* da16, const void* u16, void* du16, float* dbias, int rows, int dim, int bf16, cudaStream_t stream) {
   B200_REQUIRE(rows > 0 && dim > 0 && dim % 8 == 0, B200_ERR_SHAPE, "gelu_bwd: dim %d must be a multiple of 8", dim);
   B200_REQUIRE(ALIGNED16(da16) && ALIGNED16(u16) && ALIGNED16(du16), B200_ERR_ALIGN, "gelu_bwd: pointers must be 16-byte aligned");
-  static const int rs = env_int("B200_TRAIN_RS_GELU", 32), dbg = env_int("B200_TRAIN_DBG", 0);
-  dim3 grid((dim / 8 + 127) / 128, (rows + rs - 1) / rs);
+  dim3 grid((dim / 8 + 127) / 128, (rows + kGeluBwdRowsPerLane - 1) / kGeluBwdRowsPerLane);
   const uint16_t *a = static_cast<const uint16_t*>(da16), *u = static_cast<const uint16_t*>(u16);
-  if (bf16) gelu_bwd_kernel<true><<<grid, 128, 0, stream>>>(a, u, static_cast<uint16_t*>(du16), dbias, rows, dim, rs, dbg);
-  else gelu_bwd_kernel<false><<<grid, 128, 0, stream>>>(a, u, static_cast<uint16_t*>(du16), dbias, rows, dim, rs, dbg);
+  if (bf16) gelu_bwd_kernel<true><<<grid, 128, 0, stream>>>(a, u, static_cast<uint16_t*>(du16), dbias, rows, dim);
+  else gelu_bwd_kernel<false><<<grid, 128, 0, stream>>>(a, u, static_cast<uint16_t*>(du16), dbias, rows, dim);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;
 }
 
 int launch_gate_bwd(const float* dx, const void* m16, const float* gate, long long gate_bs, int rows_per_batch, void* dm16,
                     float* dgate, long long dgate_bs, float* dbias, int rows, int dim, int bf16, cudaStream_t stream) {
-  static const int rs_env = env_int("B200_TRAIN_RS_GATE", 32), dbg = env_int("B200_TRAIN_DBG", 0);
-  const int rs = rs_env > 0 ? rs_env : 32;
   B200_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && rows_per_batch > 0 && gate_bs % 4 == 0, B200_ERR_SHAPE, "gate_bwd: bad shape");
   B200_REQUIRE(ALIGNED16(dx) && ALIGNED16(gate) && (reinterpret_cast<uintptr_t>(m16) & 7) == 0 && (reinterpret_cast<uintptr_t>(dm16) & 7) == 0,
                B200_ERR_ALIGN, "gate_bwd: misaligned pointer");
   const int batch = (rows + rows_per_batch - 1) / rows_per_batch;
-  dim3 grid((dim / 4 + 127) / 128, (rows_per_batch + rs - 1) / rs, batch);
+  dim3 grid((dim / 4 + 127) / 128, (rows_per_batch + kGateBwdRowsPerLane - 1) / kGateBwdRowsPerLane, batch);
   const uint16_t* m = static_cast<const uint16_t*>(m16);
-  if (bf16) gate_bwd_kernel<true><<<grid, 128, 0, stream>>>(dx, m, gate, gate_bs, rows_per_batch, static_cast<uint16_t*>(dm16), dgate, dgate_bs, dbias, rows, dim, rs, dbg);
-  else gate_bwd_kernel<false><<<grid, 128, 0, stream>>>(dx, m, gate, gate_bs, rows_per_batch, static_cast<uint16_t*>(dm16), dgate, dgate_bs, dbias, rows, dim, rs, dbg);
+  if (bf16) gate_bwd_kernel<true><<<grid, 128, 0, stream>>>(dx, m, gate, gate_bs, rows_per_batch, static_cast<uint16_t*>(dm16), dgate, dgate_bs, dbias, rows, dim);
+  else gate_bwd_kernel<false><<<grid, 128, 0, stream>>>(dx, m, gate, gate_bs, rows_per_batch, static_cast<uint16_t*>(dm16), dgate, dgate_bs, dbias, rows, dim);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;
 }
@@ -1447,11 +1154,10 @@ int launch_gate_bwd(const float* dx, const void* m16, const float* gate, long lo
 int launch_colsum(const void* a, int dtype, float* out, int rows, int dim, cudaStream_t stream) {
   B200_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && dtype >= 0 && dtype <= 2, B200_ERR_SHAPE, "colsum: bad shape / dtype");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(a) & (dtype == 0 ? 15 : 7)) == 0, B200_ERR_ALIGN, "colsum: misaligned input");
-  static const int rs = env_int("B200_TRAIN_RS_COLSUM", 64);
-  dim3 grid((dim / 4 + 127) / 128, (rows + rs - 1) / rs);
-  if (dtype == 0) colsum_kernel<0><<<grid, 128, 0, stream>>>(a, out, rows, dim, rs);
-  else if (dtype == 1) colsum_kernel<1><<<grid, 128, 0, stream>>>(a, out, rows, dim, rs);
-  else colsum_kernel<2><<<grid, 128, 0, stream>>>(a, out, rows, dim, rs);
+  dim3 grid((dim / 4 + 127) / 128, (rows + kColsumRowsPerLane - 1) / kColsumRowsPerLane);
+  if (dtype == 0) colsum_kernel<0><<<grid, 128, 0, stream>>>(a, out, rows, dim);
+  else if (dtype == 1) colsum_kernel<1><<<grid, 128, 0, stream>>>(a, out, rows, dim);
+  else colsum_kernel<2><<<grid, 128, 0, stream>>>(a, out, rows, dim);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;
 }
@@ -1459,14 +1165,11 @@ int launch_colsum(const void* a, int dtype, float* out, int rows, int dim, cudaS
 template <bool BF16, int NV>
 static int lnb_launch(cudaStream_t stream, const uint16_t* dh, const float* x, const float* scale, long long mod_bs, int rpb, float* dx,
                       float* dshift, float* dscale, long long dmod_bs, int rows, int dim) {
-  auto kern = ln_modulate_bwd_kernel<BF16, NV>;
-  static const int warps = env_int("B200_LNB_WARPS", 4), rpw_env = env_int("B200_LNB_RPW", 8), dbg = env_int("B200_TRAIN_DBG", 0);
-  const int nw = (warps == 8 || warps == 2) ? warps : 4, rpw = rpw_env > 0 ? rpw_env : 8;
-  const size_t smem = static_cast<size_t>(dim) * 2 * nw * sizeof(float);
-  B200_SET_SMEM_ONCE(kern, static_cast<int>(static_cast<size_t>(dim) * 16 * sizeof(float)));
+  // [warps][2][dim] fp32 column sums: at most 48 KiB for dim <= 1536, within the default dynamic shared memory limit
+  const size_t smem = static_cast<size_t>(dim) * 2 * kLnbWarps * sizeof(float);
   const int batch = (rows + rpb - 1) / rpb;
-  dim3 grid((rpb + nw * rpw - 1) / (nw * rpw), batch);
-  kern<<<grid, nw * 32, smem, stream>>>(dh, x, scale, mod_bs, rpb, dx, dshift, dscale, dmod_bs, rows, dim, rpw, dbg);
+  dim3 grid((rpb + kLnbWarps * kLnbRowsPerWarp - 1) / (kLnbWarps * kLnbRowsPerWarp), batch);
+  ln_modulate_bwd_kernel<BF16, NV><<<grid, kLnbWarps * 32, smem, stream>>>(dh, x, scale, mod_bs, rpb, dx, dshift, dscale, dmod_bs, rows, dim);
   B200_CHECK_CUDA(cudaGetLastError());
   return B200_OK;
 }
@@ -1535,30 +1238,22 @@ int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* 
     if (bf16) return attn_bwd_two_pass<true, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
     return attn_bwd_two_pass<false, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
   }
-  if (temporal) {
-    B200_REQUIRE(frames <= 16 && head_dim % 8 == 0 && head_dim <= 128, B200_ERR_UNSUPPORTED, "attention_bwd: temporal sequences of <= 16 frames, head_dim %% 8 == 0 (got %d, %d)", frames, head_dim);
-    if (head_dim == 64 || head_dim == 72) {       // tensor-core kernel: one warp per (b, n, head)
-      const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(head_dim));
-      dim3 grid_w(batch * tokens, (heads + 3) / 4);
-      const int hdp = (head_dim + 15) / 16 * 16 + 8;
-      const size_t smem_w = static_cast<size_t>(4) * (4 * 16 * hdp + 64) * 2;
+  if (temporal) {                                 // 1..16 frames: one warp per (b, n, head) on tensor cores
+    B200_REQUIRE(head_dim == 64 || head_dim == 72, B200_ERR_UNSUPPORTED,
+                 "attention_bwd: temporal sequences of 1..16 frames need head_dim 64 or 72 (got %d frames, head_dim %d)", frames, head_dim);
+    const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(head_dim));
+    dim3 grid_w(batch * tokens, (heads + 3) / 4);
+    const int hdp = (head_dim + 15) / 16 * 16 + 8;
+    const size_t smem_w = static_cast<size_t>(4) * (4 * 16 * hdp + 64) * 2;
 #define TMMA(BF, HDV)                                                                                                          \
-      do {                                                                                                                      \
-        auto kern = attn_bwd_temporal_mma_kernel<BF, HDV>;                                                                      \
-        B200_SET_SMEM_ONCE(kern, static_cast<int>(smem_w));                                                                     \
-        kern<<<grid_w, 128, smem_w, stream>>>(q, g, dq, frames, tokens, heads, scale_log2);                                     \
-      } while (0)
-      if (head_dim == 72) { if (bf16) TMMA(true, 72); else TMMA(false, 72); }
-      else { if (bf16) TMMA(true, 64); else TMMA(false, 64); }
+    do {                                                                                                                        \
+      auto kern = attn_bwd_temporal_mma_kernel<BF, HDV>;                                                                        \
+      B200_SET_SMEM_ONCE(kern, static_cast<int>(smem_w));                                                                       \
+      kern<<<grid_w, 128, smem_w, stream>>>(q, g, dq, frames, tokens, heads, scale_log2);                                       \
+    } while (0)
+    if (head_dim == 72) { if (bf16) TMMA(true, 72); else TMMA(false, 72); }
+    else { if (bf16) TMMA(true, 64); else TMMA(false, 64); }
 #undef TMMA
-      B200_CHECK_CUDA(cudaGetLastError());
-      return B200_OK;
-    }
-    const size_t smem = (static_cast<size_t>(4) * frames * (head_dim + 1) + 2 * frames * frames) * sizeof(float);
-    const float scale = 1.0f / sqrtf(static_cast<float>(head_dim));
-    dim3 grid(batch * tokens, heads);
-    if (bf16) attn_bwd_temporal_kernel<true><<<grid, 128, smem, stream>>>(q, g, dq, frames, tokens, heads, head_dim, scale);
-    else attn_bwd_temporal_kernel<false><<<grid, 128, smem, stream>>>(q, g, dq, frames, tokens, heads, head_dim, scale);
     B200_CHECK_CUDA(cudaGetLastError());
     return B200_OK;
   }

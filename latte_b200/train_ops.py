@@ -60,24 +60,19 @@ class NativeOps:
             return dW32
         return self.linear_accum(dW32, self.transpose(dy), self.transpose(x))
 
-    def dgrad(self, dy, w, gelu_u=None):
-        """dx [rows, n_in] = dy [rows, n_out] @ w [n_out, n_in] with the weight in its nn.Linear layout (MN-major W operand);
-        with `gelu_u` the epilogue multiplies by gelu_tanh'(gelu_u) (the backward through the Mlp activation)."""
-        self._cuda(dy, w, gelu_u)
+    def dgrad(self, dy, w):
+        """dx [rows, n_in] = dy [rows, n_out] @ w [n_out, n_in] with the weight in its nn.Linear layout (MN-major W operand)."""
+        self._cuda(dy, w)
         rows, n_out = dy.shape
         n_in = w.shape[1]
         if n_in % 128 == 0 and n_out % 64 == 0:
-            assert dy.is_contiguous() and w.is_contiguous() and dy.dtype == w.dtype and (gelu_u is None or gelu_u.is_contiguous())
+            assert dy.is_contiguous() and w.is_contiguous() and dy.dtype == w.dtype
             dx = torch.empty(rows, n_in, dtype=dy.dtype, device=dy.device)
             with torch.cuda.device(dy.device):
-                rc = _lib.load().b200_dgrad(dy.data_ptr(), w.data_ptr(), gelu_u.data_ptr() if gelu_u is not None else None, dx.data_ptr(),
-                                            rows, n_out, n_in, self.dt, _s(dy))
+                rc = _lib.load().b200_dgrad(dy.data_ptr(), w.data_ptr(), dx.data_ptr(), rows, n_out, n_in, self.dt, _s(dy))
             _lib.check(rc, "b200_dgrad")
             return dx
-        dx = self.linear(dy, self.transpose(w))
-        if gelu_u is None:
-            return dx
-        return self.gelu_bwd(dx, gelu_u, torch.zeros(n_in, dtype=torch.float32, device=dy.device))
+        return self.linear(dy, self.transpose(w))
 
     def linear_gelu_both(self, a, w, bias):
         """(u, gelu_tanh(u)) with u = a @ w^T + bias, both from one GEMM epilogue (training-mode fc1)."""
@@ -107,28 +102,6 @@ class NativeOps:
                                                 out.data_ptr(), x.shape[0], x.shape[1], self.dt, _s(x))
         _lib.check(rc, "b200_gate_residual")
         return out
-
-    def gate_residual_ln(self, x, m, gate, shift, scale, rpb, row_add=None, tokens=1):
-        """(x_out, h) = (x + gate * m (+ row_add), LN-modulate(x_out)) in one pass."""
-        self._cuda(x, m, gate, shift, scale, row_add)
-        assert x.dtype == torch.float32 and x.is_contiguous() and m.is_contiguous() and shift.stride(0) == scale.stride(0)
-        out = torch.empty_like(x)
-        h = torch.empty(x.shape, dtype=self.dtype, device=x.device)
-        frames = row_add.shape[0] if row_add is not None else 0
-        with torch.cuda.device(x.device):
-            rc = _lib.load().b200_gate_residual_ln(x.data_ptr(), m.data_ptr(), gate.data_ptr(), gate.stride(0), shift.data_ptr(), scale.data_ptr(),
-                                                   shift.stride(0), rpb, row_add.data_ptr() if row_add is not None else None, tokens, frames,
-                                                   out.data_ptr(), h.data_ptr(), x.shape[0], x.shape[1], self.dt, _s(x))
-        _lib.check(rc, "b200_gate_residual_ln")
-        return out, h
-
-    def gelu(self, u):
-        self._cuda(u)
-        a = torch.empty_like(u)
-        with torch.cuda.device(u.device):
-            rc = _lib.load().b200_gelu(u.data_ptr(), a.data_ptr(), u.numel(), self.dt, _s(u))
-        _lib.check(rc, "b200_gelu")
-        return a
 
     # ------------------------------------------------------------------ backward ops
     # Reduction outputs (dgate, dbias, dshift, dscale, column sums) ACCUMULATE into the fp32 views the engine hands in -- slices of
@@ -194,14 +167,8 @@ class NativeOps:
         return out
 
     def cast(self, w32):
-        self._cuda(w32)
-        w32 = w32.detach().float().contiguous()
-        R, Cc = w32.shape
-        w = torch.empty(R, Cc, dtype=self.dtype, device=w32.device)
-        with torch.cuda.device(w32.device):
-            rc = _lib.load().b200_cast_transpose(w32.data_ptr(), w.data_ptr(), None, R, Cc, self.dt, _s(w32))
-        _lib.check(rc, "b200_cast_transpose")
-        return w
+        """A fresh 16-bit copy of a parameter."""
+        return self.to_operand(w32.detach().float())
 
     def cast_into(self, srcs, dsts):
         """dsts[i] (16-bit, contiguous) = srcs[i] (fp32, contiguous) for all i in ONE launch; the pointer table is cached for as

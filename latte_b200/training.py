@@ -17,12 +17,9 @@ gradients produced by the unmodified reference (tests/golden/train_tiny64.npz).
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 _BLOCK_LINEARS = ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")
-_FUSED_RESIDUAL_LN = os.environ.get("LATTE_B200_FUSED_RESIDUAL_LN", "0") == "1"
 
 
 class TrainEngine:
@@ -145,14 +142,9 @@ class TrainEngine:
             qkv = ops.linear(h1, wq[0], wq[1])
             o = ops.attention(qkv, B, Fr, N, H, temporal)
             m1 = ops.linear(o, wp[0], wp[1])
-            # (`ops.gate_residual_ln` does the residual update and the next LayerNorm-modulate in one pass; built and tested, but
-            # timed alone it is slower than the two tuned passes it replaces (101 vs 45 + 40 us), so it is off by default;
-            # LATTE_B200_FUSED_RESIDUAL_LN=1 switches it on for this half of the block for A/B runs)
-            if _FUSED_RESIDUAL_LN:
-                xm, h2 = ops.gate_residual_ln(xs, m1, g1, sh2, sc2, rpb)
-            else:
-                xm = ops.gate_residual(xs, m1, g1, rpb)
-                h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
+            # two passes: a kernel fusing the residual update with this LayerNorm-modulate measured slower (101 vs 45 + 40 us)
+            xm = ops.gate_residual(xs, m1, g1, rpb)
+            h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
             u, a = ops.linear_gelu_both(h2, w1[0], w1[1])
             m2 = ops.linear(a, w2[0], w2[1])
             xo = ops.gate_residual(xm, m2, g2, rpb, row_add=temp if i == 0 else None, tokens=N)
@@ -222,8 +214,7 @@ class TrainEngine:
             dm2 = ops.gate_bwd(dx, m2, g2, rpb, dg2, G[p + "mlp.fc2.bias"])
             G[p + "mlp.fc2.weight"] = wgrad(dm2, a)
             del a
-            # gelu'(u) stays a separate pass: as an epilogue of this dgrad (`gelu_u=u`, built and tested) it made the N = 4608
-            # epilogue the bottleneck of the GEMM -- 327 us against 153 + 129 us for dgrad + gelu_bwd (which also sums the bias gradient)
+            # gelu'(u) is a separate pass: in this dgrad's epilogue it made the GEMM the bottleneck (327 us vs 153 + 129 us)
             da = ops.dgrad(dm2, w2[0])
             du = ops.gelu_bwd(da, u, G[p + "mlp.fc1.bias"])
             del da, dm2

@@ -46,12 +46,9 @@ class TorchOps:
         out32 += r
         return out32
 
-    def dgrad(self, dy, w, gelu_u=None):
-        """dx [rows, n_in] = dy [rows, n_out] @ w [n_out, n_in]; with gelu_u: times gelu_tanh'(gelu_u) (the rounded dx, like the kernel)."""
-        dx = (dy.float() @ w.float()).to(self.dtype)
-        if gelu_u is None:
-            return dx
-        return self.gelu_bwd(dx, gelu_u, torch.zeros(w.shape[1], dtype=torch.float32, device=dy.device))
+    def dgrad(self, dy, w):
+        """dx [rows, n_in] = dy [rows, n_out] @ w [n_out, n_in]."""
+        return (dy.float() @ w.float()).to(self.dtype)
 
     def linear_gelu_both(self, a, w, bias):
         u = self.linear(a, w, bias)
@@ -94,10 +91,6 @@ class TorchOps:
             Fr = row_add.shape[0]
             out = out.view(B, Fr, tokens, -1) + row_add.float()[None, :, None]
         return out.reshape(x.shape).contiguous()
-
-    def gate_residual_ln(self, x, m, gate, shift, scale, rpb, row_add=None, tokens=1):
-        out = self.gate_residual(x, m, gate, rpb, row_add=row_add, tokens=tokens)
-        return out, self.ln_modulate(out, shift, scale, rpb)
 
     def gelu(self, u):
         return F.gelu(u.float(), approximate="tanh").to(self.dtype)

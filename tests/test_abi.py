@@ -59,6 +59,29 @@ def test_sass_is_hopper_native():
     assert all("attn_bwd" in n for n in legacy), f"legacy mma.sync outside the attention backward: {sorted(legacy)[:4]}"
 
 
+def test_exports_are_exactly_the_header(lib):
+    """The library's dynamic symbol table holds exactly the b200_* entry points the header declares: nothing removed from
+    the ABI lingers in the binary."""
+    import shutil
+    import subprocess
+    from latte_b200 import _lib
+    nm = shutil.which("nm")
+    if nm is None:
+        pytest.skip("nm not available")
+    out = subprocess.run([nm, "-D", "--defined-only", _lib.lib_path()], capture_output=True, text=True, check=True).stdout
+    exported = sorted({line.split()[-1] for line in out.splitlines() if line.split() and line.split()[-1].startswith("b200_")})
+    assert exported == _header_symbols()
+
+
+def test_library_reads_no_environment():
+    """No code path of the library or the training engine is selected by an environment variable."""
+    csrc = os.path.join(ROOT, "latte_b200", "csrc")
+    readers = [f for f in sorted(os.listdir(csrc)) if os.path.isfile(os.path.join(csrc, f)) and
+               "getenv" in open(os.path.join(csrc, f), encoding="utf-8", errors="replace").read()]
+    assert readers == []
+    assert "os.environ" not in open(os.path.join(ROOT, "latte_b200", "training.py")).read()
+
+
 def test_abi_version_and_error_text(lib):
     from latte_b200 import _lib
     assert lib.b200_abi_version() == _lib.ABI_VERSION

@@ -105,17 +105,6 @@ def _attn_ref(qkv, batch, frames, tokens, heads, temporal):
     return o.reshape(T, D)
 
 
-@pytest.fixture(params=[2, 3], ids=["attn_v2", "attn_v3"])
-def attn_impl(request):
-    """Every attention test runs through b200_set_attention_impl (include/latte_b200.h) with both non-default values the ABI
-    accepts; the sm_90a build has one attention kernel, so both select it -- the switch must keep accepting them."""
-    from latte_b200 import _lib
-    lib = _lib.load()
-    _lib.check(lib.b200_set_attention_impl(request.param), "b200_set_attention_impl")
-    yield request.param
-    lib.b200_set_attention_impl(0)
-
-
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("case", [
     (2, 16, 256, 16, 72, False), (2, 16, 256, 16, 72, True),      # XL/2 spatial / temporal
@@ -124,7 +113,7 @@ def attn_impl(request):
     (2, 8, 64, 2, 64, True), (4, 4, 64, 8, 72, True), (1, 32, 32, 2, 80, True),      # F = 8, 4, 32; head_dim 80
     (1, 2, 512, 2, 64, False), (1, 2, 1024, 4, 72, False), (2, 16, 1024, 2, 72, True),  # LatteT2V @512px: N = 1024 (online softmax)
 ])
-def test_attention(dev, dt, case, attn_impl):
+def test_attention(dev, dt, case):
     from latte_b200 import ops
     b, f, n, h, hd, temporal = case
     g = torch.Generator().manual_seed(b * 1000 + f * 10 + n + hd)
@@ -132,7 +121,7 @@ def test_attention(dev, dt, case, attn_impl):
     _close(ops.attention(qkv, b, f, n, h, temporal), _attn_ref(qkv, b, f, n, h, temporal), TOL[dt])
 
 
-def test_attention_properties(dev, attn_impl):
+def test_attention_properties(dev):
     """V = 1 -> out = 1; Q = 0 -> out = mean of V over the sequence; permuting the keys of a sequence leaves the output unchanged."""
     from latte_b200 import ops
     b, f, n, h, hd = 1, 16, 256, 16, 72
@@ -179,7 +168,7 @@ def test_ln_modulate(dev, dt, D):
 
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("case", [(2, 256, 120, 4, 72), (1, 1024, 20, 2, 64), (3, 128, 128, 2, 80), (2, 512, 1, 4, 72)])
-def test_cross_attention(dev, dt, case, attn_impl):
+def test_cross_attention(dev, dt, case):
     """diffusers Attention (attn2) with text keys (latte_t2v.py:862-870): q from the video tokens, k/v from <=128 text tokens."""
     from latte_b200 import ops
     b, rows, L, h, hd = case
@@ -197,7 +186,7 @@ def test_cross_attention(dev, dt, case, attn_impl):
 
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("case", [(2, 256, 120, 4, 72, (12, 120)), (3, 128, 20, 2, 64, (1, 20, 7)), (2, 1024, 128, 2, 80, (128, 3))])
-def test_cross_attention_key_bias(dev, dt, case, attn_impl):
+def test_cross_attention_key_bias(dev, dt, case):
     """Padded prompts (latte_t2v.py:766-771): the keep-mask becomes the additive bias (1 - m) * -10000 on the scores."""
     from latte_b200 import ops
     b, rows, L, h, hd, valid = case

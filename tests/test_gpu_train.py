@@ -118,15 +118,6 @@ def test_elementwise_forward_ops(dev, dt):
     _close(nat.gate_residual(x, m, gate, rpb), ref.gate_residual(x, m, gate, rpb), 1e-6, "gate_residual")
     _close(nat.gate_residual(x, m, gate, rpb, row_add=temp, tokens=N), ref.gate_residual(x, m, gate, rpb, row_add=temp, tokens=N),
            1e-6, "gate_residual+temp")
-    u = (torch.randn(T, 4 * D, generator=g) * 2).to(dev).to(dt)
-    _close(nat.gelu(u), ref.gelu(u), EPS[dt], "gelu")
-    # the residual update and the LayerNorm-modulate that follows it, fused
-    shift, scale = mod[:, 3 * D:4 * D], mod[:, 4 * D:5 * D]
-    for kw in (dict(), dict(row_add=temp, tokens=N)):
-        xo, h = nat.gate_residual_ln(x, m, gate, shift, scale, rpb, **kw)
-        xo_r, h_r = ref.gate_residual_ln(x, m, gate, shift, scale, rpb, **kw)
-        _close(xo, xo_r, 1e-6, "gate_residual_ln x_out")
-        _close(h, h_r, EPS[dt], "gate_residual_ln h")
 
 
 @pytest.mark.parametrize("dt", DTS)
@@ -199,7 +190,7 @@ def test_adaln_gradients(dev, dt):
 
 @pytest.mark.parametrize("dt", DTS)
 def test_fused_gelu_epilogues(dev, dt):
-    """Training-mode fc1 (u and gelu(u) from one epilogue) and the dgrad of fc2 with gelu'(u) in its epilogue."""
+    """Training-mode fc1: u and gelu(u) from one epilogue."""
     nat, ref = _ops(dt)
     g = torch.Generator().manual_seed(12)
     a = torch.randn(2048, 384, generator=g).to(dev).to(dt)
@@ -210,9 +201,6 @@ def test_fused_gelu_epilogues(dev, dt):
     _close(u, u_r, EPS[dt], "fc1 pre-activation")
     _close(act, ref.gelu(u), EPS[dt], "gelu of the kernel's own u")
     _close(act, act_r, 2 * EPS[dt], "gelu(u)")
-    dy = torch.randn(2048, 384, generator=g).to(dev).to(dt)
-    w2 = (torch.randn(384, 1536, generator=g) / 384 ** 0.5).to(dev).to(dt)
-    _close(nat.dgrad(dy, w2, gelu_u=u), ref.dgrad(dy, w2, gelu_u=u), 2 * EPS[dt], "dgrad * gelu'(u)")
 
 
 def test_fused_training_loss_matches_torch_expressions(dev):

@@ -98,11 +98,12 @@ def test_temporal_backward_stale_nan_and_nan_sequence(dev, dt, frames):
 
 def test_temporal_backward_head_dim_80_is_unsupported(dev):
     nat, _ = _ops(torch.bfloat16)
-    B, Fr, N, H, hd = 1, 32, 2, 2, 80
-    qkv, do = _inputs(dev, torch.bfloat16, B, Fr, N, H, hd, 3)
-    o = torch.zeros_like(do)
-    with pytest.raises(RuntimeError, match="UNSUPPORTED"):
-        nat.attention_bwd(qkv, o, do, B, Fr, N, H, True)
+    B, N, H, hd = 1, 2, 2, 80
+    for Fr in (8, 32):                     # the one-warp kernel (<= 16 frames) and the strided two-kernel path
+        qkv, do = _inputs(dev, torch.bfloat16, B, Fr, N, H, hd, 3)
+        o = torch.zeros_like(do)
+        with pytest.raises(RuntimeError, match="UNSUPPORTED"):
+            nat.attention_bwd(qkv, o, do, B, Fr, N, H, True)
 
 
 @pytest.mark.parametrize("dt", DTS)

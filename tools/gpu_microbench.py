@@ -64,32 +64,22 @@ def attn():
     g = torch.Generator().manual_seed(1)
     b, f, n, h, hd = 2, 16, 256, 16, 72
     qkv = torch.randn(b * f * n, 3 * h * hd, generator=g).to(dev).half()
-    from latte_b200 import _lib
-    lib = _lib.load()
-    for impl in [int(v) for v in os.environ.get('B200_MB_IMPLS', '2,3').split(',')]:
-        lib.b200_set_attention_impl(impl)
-        for temporal in (False, True):
-            for fl_on in (True, False):
-                best, mean = bench(lambda: ops.attention(qkv, b, f, n, h, temporal), do_flush=fl_on)
-                byts = qkv.numel() * 2 + b * f * n * h * hd * 2
-                flops = 4.0 * (f * f * n if temporal else n * n * f) * h * hd * b
-                print(f"attn v{impl} {'temporal' if temporal else 'spatial '} {'cold' if fl_on else 'warm'}: best {best:7.1f} us mean {mean:7.1f} -> {byts / best / 1e3:7.1f} GB/s, {flops / best / 1e6:6.1f} TFLOP/s", flush=True)
-    lib.b200_set_attention_impl(0)
+    for temporal in (False, True):
+        for fl_on in (True, False):
+            best, mean = bench(lambda: ops.attention(qkv, b, f, n, h, temporal), do_flush=fl_on)
+            byts = qkv.numel() * 2 + b * f * n * h * hd * 2
+            flops = 4.0 * (f * f * n if temporal else n * n * f) * h * hd * b
+            print(f"attn {'temporal' if temporal else 'spatial '} {'cold' if fl_on else 'warm'}: best {best:7.1f} us mean {mean:7.1f} -> {byts / best / 1e3:7.1f} GB/s, {flops / best / 1e6:6.1f} TFLOP/s", flush=True)
 
 
 def attn_long():
     """LatteT2V @512 px: spatial attention over N = 1024 tokens per frame (B_model = 2, 16 frames, 16 heads x 72)."""
-    from latte_b200 import _lib
-    lib = _lib.load()
     g = torch.Generator().manual_seed(3)
     b, f, n, h, hd = 2, 16, 1024, 16, 72
     qkv = torch.randn(b * f * n, 3 * h * hd, generator=g).to(dev).half()
-    for impl in [int(v) for v in os.environ.get('B200_MB_IMPLS', '2,3').split(',')]:
-        lib.b200_set_attention_impl(impl)
-        best, mean = bench(lambda: ops.attention(qkv, b, f, n, h, False), iters=10)
-        flops = 4.0 * n * n * f * h * hd * b
-        print(f"attn N=1024 v{impl}: best {best:7.1f} us mean {mean:7.1f} -> {flops / best / 1e6:6.1f} TFLOP/s", flush=True)
-    lib.b200_set_attention_impl(0)
+    best, mean = bench(lambda: ops.attention(qkv, b, f, n, h, False), iters=10)
+    flops = 4.0 * n * n * f * h * hd * b
+    print(f"attn N=1024: best {best:7.1f} us mean {mean:7.1f} -> {flops / best / 1e6:6.1f} TFLOP/s", flush=True)
 
 
 def ln():

@@ -8,7 +8,7 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from latte_b200 import Latte, LatteT2V, _lib, ops  # noqa: E402
+from latte_b200 import Latte, LatteT2V, ops  # noqa: E402
 from oracle import latte_oracle as O  # noqa: E402
 
 dev = torch.device("cuda:0")
@@ -50,24 +50,20 @@ def gemm():
 
 
 def attn():
-    lib = _lib.load()
     g = torch.Generator().manual_seed(1)
-    for impl in (2, 3):
-        lib.b200_set_attention_impl(impl)
-        for (b, f, n, h, hd, temporal) in [(1, 2, 256, 2, 72, False), (1, 16, 16, 2, 72, True), (1, 8, 32, 2, 64, True), (1, 2, 64, 2, 80, False),
-                                           (1, 1, 128, 1, 64, False)]:
-            qkv = torch.randn(b * f * n, 3 * h * hd, generator=g).to(dev).half()
-            o = ops.attention(qkv, b, f, n, h, temporal)
-            torch.cuda.synchronize()
-            print(f"attn v{impl} b{b} f{f} n{n} h{h} hd{hd} temporal={temporal}: finite", bool(torch.isfinite(o.float()).all()), flush=True)
-        q = torch.randn(2 * 128, 2 * 72, generator=g).to(dev).half()
-        kv = torch.randn(2 * 20, 2 * 2 * 72, generator=g).to(dev).half()
-        bias = torch.zeros(2, 128)
-        bias[0, 5:] = -10000.0
-        o = ops.cross_attention(q, kv, 2, 128, 20, 2, key_bias=bias.to(dev))
+    for (b, f, n, h, hd, temporal) in [(1, 2, 256, 2, 72, False), (1, 16, 16, 2, 72, True), (1, 8, 32, 2, 64, True), (1, 2, 64, 2, 80, False),
+                                       (1, 1, 128, 1, 64, False)]:
+        qkv = torch.randn(b * f * n, 3 * h * hd, generator=g).to(dev).half()
+        o = ops.attention(qkv, b, f, n, h, temporal)
         torch.cuda.synchronize()
-        print(f"cross attn v{impl} with key bias: finite", bool(torch.isfinite(o.float()).all()), flush=True)
-    lib.b200_set_attention_impl(0)
+        print(f"attn b{b} f{f} n{n} h{h} hd{hd} temporal={temporal}: finite", bool(torch.isfinite(o.float()).all()), flush=True)
+    q = torch.randn(2 * 128, 2 * 72, generator=g).to(dev).half()
+    kv = torch.randn(2 * 20, 2 * 2 * 72, generator=g).to(dev).half()
+    bias = torch.zeros(2, 128)
+    bias[0, 5:] = -10000.0
+    o = ops.cross_attention(q, kv, 2, 128, 20, 2, key_bias=bias.to(dev))
+    torch.cuda.synchronize()
+    print("cross attn with key bias: finite", bool(torch.isfinite(o.float()).all()), flush=True)
     qkv = torch.randn(1 * 1 * 512, 3 * 1 * 72, generator=g).to(dev).half()     # N = 512: the online-softmax kernel
     o = ops.attention(qkv, 1, 1, 512, 1, False)
     torch.cuda.synchronize()

@@ -27,6 +27,5 @@ for rep in range(2):
     ops.gate_bwd(dx, m16, mod[:, 2 * D:3 * D], rpb, dmod[:, 2 * D:3 * D], db[:D])
     ops.gelu_bwd(da, u, db)
     ops.colsum(qkv, db[:3 * D])
-    ops.gate_residual_ln(x, m16, mod[:, 2 * D:3 * D], mod[:, :D], mod[:, D:2 * D], rpb)
 torch.cuda.synchronize()
 print("done")
