@@ -3,12 +3,20 @@
 `sample/sample.py:56`, `sample/sample_ddp.py:88` and `train.py:90` call `get_models(args)`; putting this
 package ahead of the reference's on sys.path (see INTEGRATION.md) swaps the denoiser and nothing else."""
 from latte_b200.latte import Latte, Latte_models  # noqa: F401  (absolute: also importable as top-level `models` via a symlink)
+from latte_b200.latte_img import LatteIMG, LatteIMG_models  # noqa: F401
 
 
 def get_models(args):
     name = args.model
     if "LatteIMG" in name:
-        raise NotImplementedError("LatteIMG (video+image joint training variant, models/latte_img.py) is not built")
+        # models/__init__.py:32-38 (train_with_img.py).  The conditioning is checked first: extras=78 (the legacy CLIP text
+        # projection) is not built, and neither is an argument set that names no conditioning at all.
+        extras = getattr(args, "extras", None)
+        if extras not in (1, 2):
+            raise NotImplementedError(f"{name} with extras={extras!r}: LatteIMG is built for extras=2 (class labels, per-image "
+                                      "labels in training) and extras=1 (timestep only)")
+        return LatteIMG_models[name](input_size=args.latent_size, num_classes=args.num_classes,
+                                     num_frames=args.num_frames, learn_sigma=args.learn_sigma, extras=args.extras)
     if "LatteT2V" in name:
         # models/__init__.py:40-41
         from latte_b200.latte_t2v import LatteT2V

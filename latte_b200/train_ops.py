@@ -200,8 +200,29 @@ class NativeOps:
         _lib.check(rc, "b200_cast16")
         return out
 
+    # adaLN gradients, dW = dmod^T silu(c) and dsc = dmod W_ada.  Up to 8 rows (per-sample conditioning at a small local batch)
+    # they are one pass each over the stacked weight (b200_ada_outer / b200_ada_dsc).  More rows (a large local batch, or one row
+    # per frame in video + image training) go through the weight-gradient GEMM: dmod rounded to the operand type (what the
+    # reference computes under bf16 autocast) and zero-padded to a multiple of 64 rows, fp32 reduce-add into the result.
+    _ADA_ROWS = 8
+
+    def _ada_rows16(self, dmod):
+        """dmod fp32 (R, NA) -> 16-bit (R', NA), R' = R rounded up to 64 with zero rows."""
+        R, NA = dmod.shape
+        d16 = torch.zeros((R + 63) // 64 * 64, NA, dtype=self.dtype, device=dmod.device)
+        with torch.cuda.device(dmod.device):
+            rc = _lib.load().b200_cast16(dmod.contiguous().data_ptr(), d16.data_ptr(), R * NA, self.dt, _s(dmod))
+        _lib.check(rc, "b200_cast16")
+        return d16
+
     def ada_outer(self, dmod, sc):
         self._cuda(dmod, sc)
+        if dmod.shape[0] > self._ADA_ROWS:
+            R, D = sc.shape
+            d16 = self._ada_rows16(dmod)
+            sc16 = torch.zeros(d16.shape[0], D, dtype=self.dtype, device=sc.device)
+            sc16[:R] = sc
+            return self.wgrad(torch.zeros(dmod.shape[1], D, dtype=torch.float32, device=dmod.device), d16, sc16)
         B, NA = dmod.shape
         D = sc.shape[1]
         dW = torch.empty(NA, D, dtype=torch.float32, device=dmod.device)
@@ -212,6 +233,12 @@ class NativeOps:
 
     def ada_dsc(self, dmod, w):
         self._cuda(dmod, w)
+        if dmod.shape[0] > self._ADA_ROWS:
+            # dsc^T is the weight gradient of the (NA x R') operand dmod^T against W_ada: K = NA, a long-K few-tile GEMM that the
+            # stream-K schedule spreads over all SMs
+            d16 = self._ada_rows16(dmod)
+            dsc = torch.zeros(d16.shape[0], w.shape[1], dtype=torch.float32, device=dmod.device)
+            return self.wgrad(dsc, self.transpose(d16), w)[: dmod.shape[0]]
         B, NA = dmod.shape
         D = w.shape[1]
         dsc = torch.empty(B, D, dtype=torch.float32, device=dmod.device)

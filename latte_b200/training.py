@@ -22,11 +22,25 @@ import torch
 _BLOCK_LINEARS = ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")
 
 
+def _patch_rows(x, p):
+    """(B, F, C, H, W) -> rows (b, f, gh, gw) x columns (c, i, j)."""
+    B, Fr, C, H, Wd = x.shape
+    xx = x.reshape(B * Fr, C, H // p, p, Wd // p, p).permute(0, 2, 4, 1, 3, 5)
+    return xx.reshape(B * Fr * (H // p) * (Wd // p), C * p * p)
+
+
 class TrainEngine:
-    def __init__(self, model, ops, dtype):
+    """`images` = I still frames per sample after the F = num_frames video frames (LatteIMG, latte_img.py:316-399).  With I > 0
+    the rows of all video frames come first, in (b, f, n) order (T_v = B*F*N rows), then the rows of all images in (b, i, n)
+    order.  Spatial blocks and the final layer run over every row with one adaLN row per frame (rows_per_batch = N); temporal
+    blocks run on the prefix x[:T_v] -- exactly a Latte batch of B videos -- with one adaLN row per video (a strided view of the
+    per-frame rows), and carry the image rows through unchanged."""
+
+    def __init__(self, model, ops, dtype, images=0):
         self.m = model
         self.ops = ops
         self.dtype = dtype
+        self.images = images
         self.saved = None
         self.w = None
 
@@ -89,66 +103,115 @@ class TrainEngine:
 
     # ---------------------------------------------------------------------------------------------------------------
     def _patchify(self, x):
-        """(B, F, C, H, W) -> rows (b, f, gh, gw) x columns (c, i, j): timm PatchEmbed's Conv2d(k = s = p) as a GEMM operand."""
-        m = self.m
-        B, Fr, C, H, Wd = x.shape
-        p = m.patch_size
-        xx = x.reshape(B * Fr, C, H // p, p, Wd // p, p).permute(0, 2, 4, 1, 3, 5)
-        return xx.reshape(B * Fr * (H // p) * (Wd // p), C * p * p)
+        """(B, F[+I], C, H, W) -> rows (b, f, gh, gw) [then (b, i, gh, gw)] x columns (c, i, j): timm PatchEmbed's
+        Conv2d(k = s = p) as a GEMM operand."""
+        p, Fr = self.m.patch_size, self.m.num_frames
+        if self.images:
+            return torch.cat((_patch_rows(x[:, :Fr], p), _patch_rows(x[:, Fr:], p)))
+        return _patch_rows(x, p)
 
     def _unpatchify(self, tok, B):
-        """rows (b, f, h, w) x (p, q, c) -> (B, F, c, h*p, w*q) (latte.py:297-310, :375-376)."""
+        """rows (b, f, h, w) x (p, q, c) -> (B, F, c, h*p, w*q) (latte.py:297-310, :375-376); image rows follow as frames F.."""
         m = self.m
         c, p = m.out_channels, m.patch_size
         g = m.input_size // p
-        t = tok.view(B * m.num_frames, g, g, p, p, c).permute(0, 5, 1, 3, 2, 4)
-        return t.reshape(B, m.num_frames, c, g * p, g * p)
+
+        def unp(rows, frames):
+            t = rows.view(B * frames, g, g, p, p, c).permute(0, 5, 1, 3, 2, 4)
+            return t.reshape(B, frames, c, g * p, g * p)
+        if self.images:
+            Tv = B * m.num_frames * g * g
+            return torch.cat((unp(tok[:Tv], m.num_frames), unp(tok[Tv:], self.images)), dim=1)
+        return unp(tok, m.num_frames)
 
     def _patchify_out(self, dout):
         m = self.m
         c, p = m.out_channels, m.patch_size
         g = m.input_size // p
-        B = dout.shape[0]
-        t = dout.reshape(B * m.num_frames, c, g, p, g, p).permute(0, 2, 4, 3, 5, 1)
-        return t.reshape(B * m.num_frames * g * g, p * p * c).contiguous()
+
+        def pat(d):
+            B, frames = d.shape[:2]
+            t = d.reshape(B * frames, c, g, p, g, p).permute(0, 2, 4, 3, 5, 1)
+            return t.reshape(B * frames * g * g, p * p * c)
+        if self.images:
+            return torch.cat((pat(dout[:, :m.num_frames]), pat(dout[:, m.num_frames:])))
+        return pat(dout).contiguous()
 
     # ---------------------------------------------------------------------------------------------------------------
-    def forward(self, x, c):
-        """x (B, F, C, H, W) fp32, c (B, D) fp32 = t_embedder(t) + y_embedder(y) (latte.py:332-348) -> (B, F, 2C, H, W) fp32."""
+    def _geometry(self, B):
+        """(rows of all frames, rows of the video frames, rows_per_batch of spatial blocks / final layer, of temporal blocks)."""
+        m = self.m
+        Fr, N = m.num_frames, m.x_embedder.num_patches
+        Tv = B * Fr * N
+        if not self.images:
+            return Tv, Tv, Fr * N, Fr * N
+        return Tv + B * self.images * N, Tv, N, Fr * N
+
+    def _temporal_rows(self, t, B):
+        """The adaLN rows (of mod / dmod) a temporal block addresses: per sample without images, else the first frame's row of
+        each video (every video frame carries the same conditioning)."""
+        return t[0:B * self.m.num_frames:self.m.num_frames] if self.images else t
+
+    @staticmethod
+    def _join_rows(video, images):
+        """One buffer of the video rows followed by the image rows: the output of a temporal block, whose image rows are its
+        input's, copied device to device (B*I*N*D*4 bytes)."""
+        return torch.cat((video, images))
+
+    def forward(self, x, c, save=True):
+        """x (B, F[+I], C, H, W) fp32 -> (B, F[+I], 2C, H, W) fp32.  c: (B, D) fp32 = t_embedder(t) + y_embedder(y)
+        (latte.py:332-348) without images, else (B*(F+I), D) per-frame conditioning in row order (`frame_conditioning`).
+        save=False runs the forward without keeping the activations the backward needs."""
         if self.w is None:
             self.prepare()
         m, ops, W = self.m, self.ops, self.w
         B = x.shape[0]
         D, Fr, N, H = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads
-        T, rpb = B * Fr * N, Fr * N
+        T, Tv, rpb, rpb_t = self._geometry(B)
+        Fs = Fr + self.images                   # frames a spatial block sees
         dev = x.device
         sc = ops.to_operand(torch.nn.functional.silu(c.float()).contiguous())            # adaLN_modulation[0], final too
-        mod = ops.linear(sc, W["ada_w"], W["ada_b"]).float()                               # (B, depth*6D + 2D)
+        mod = ops.linear(sc, W["ada_w"], W["ada_b"]).float()                               # (B or B(F+I), depth*6D + 2D)
+        mod_t = self._temporal_rows(mod, B)
         S = {"B": B, "c": c, "sc": sc, "mod": mod, "blocks": []}
 
         xp = torch.zeros(T, 64, dtype=torch.float32, device=dev)
         xp[:, : self.kp] = self._patchify(x.float())
         xp = ops.to_operand(xp)
-        xs = m.pos_embed.detach().float().reshape(1, N, D).expand(B * Fr, N, D).reshape(T, D).contiguous()
+        xs = m.pos_embed.detach().float().reshape(1, N, D).expand(B * Fs, N, D).reshape(T, D).contiguous()
         ops.linear_accum(xs, xp, W["patch_w"], W["patch_b"])
-        S["xp"] = xp
+        if save:
+            S["xp"] = xp
+        del xp
         temp = m.temp_embed.detach().float().reshape(Fr, D).contiguous()
         for i in range(m.depth):
-            mv = mod[:, i * 6 * D:(i + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
             temporal = bool(i % 2)
+            mv = (mod_t if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
+            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
             wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
-            h1 = ops.ln_modulate(xs, sh1, sc1, rpb)
+            rp = rpb_t if temporal else rpb
+            xi = xs[:Tv] if temporal else xs    # temporal blocks see the video rows only (latte_img.py:373-374, 387-388)
+            h1 = ops.ln_modulate(xi, sh1, sc1, rp)
             qkv = ops.linear(h1, wq[0], wq[1])
-            o = ops.attention(qkv, B, Fr, N, H, temporal)
+            o = ops.attention(qkv, B, Fr if temporal else Fs, N, H, temporal)
             m1 = ops.linear(o, wp[0], wp[1])
             # two passes: a kernel fusing the residual update with this LayerNorm-modulate measured slower (101 vs 45 + 40 us)
-            xm = ops.gate_residual(xs, m1, g1, rpb)
-            h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
+            xm = ops.gate_residual(xi, m1, g1, rp)
+            h2 = ops.ln_modulate(xm, sh2, sc2, rp)
             u, a = ops.linear_gelu_both(h2, w1[0], w1[1])
             m2 = ops.linear(a, w2[0], w2[1])
-            xo = ops.gate_residual(xm, m2, g2, rpb, row_add=temp if i == 0 else None, tokens=N)
-            S["blocks"].append((xs, h1, qkv, o, m1, xm, h2, u, a, m2))
+            if i == 0 and self.images:
+                # temp_embed goes to the video rows only (latte_img.py:377-378).  All frames of a video share one gate row, so
+                # the video rows take the per-video view, like a temporal block.
+                g2v = mod_t[:, 5 * D:6 * D]
+                xo = self._join_rows(ops.gate_residual(xm[:Tv], m2[:Tv], g2v, rpb_t, row_add=temp, tokens=N),
+                                     ops.gate_residual(xm[Tv:], m2[Tv:], g2[B * Fr:], rp))
+            else:
+                xo = ops.gate_residual(xm, m2, g2, rp, row_add=temp if i == 0 else None, tokens=N)
+                if temporal and self.images:    # image rows pass through the temporal block unchanged
+                    xo = self._join_rows(xo, xs[Tv:])
+            if save:
+                S["blocks"].append((xi, h1, qkv, o, m1, xm, h2, u, a, m2))
             xs = xo
         base = m.depth * 6 * D
         shf, scf = mod[:, base:base + D], mod[:, base + D:base + 2 * D]
@@ -156,7 +219,7 @@ class TrainEngine:
         tok = torch.zeros(T, self.nf, dtype=torch.float32, device=dev)
         ops.linear_accum(tok, hf, W["final_w"], W["final_b"])
         S["x_last"], S["hf"] = xs, hf
-        self.saved = S
+        self.saved = S if save else None
         return self._unpatchify(tok, B)
 
     # ---------------------------------------------------------------------------------------------------------------
@@ -168,11 +231,12 @@ class TrainEngine:
         self.saved = None
         B = S["B"]
         D, Fr, N, H, Hm = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads, m.mlp_hidden
-        T, rpb = B * Fr * N, Fr * N
+        T, Tv, rpb, rpb_t = self._geometry(B)
         dev = dout.device
         mod = S["mod"]
         G = {}
         dmod = torch.zeros_like(mod)
+        mod_t, dmod_t = self._temporal_rows(mod, B), self._temporal_rows(dmod, B)
         # all bias gradients in one zeroed buffer: per block [qkv 3D | proj D | fc1 Hm | fc2 D], then final (nf), patch (D)
         per_blk = 3 * D + D + Hm + D
         bias_flat = torch.zeros(m.depth * per_blk + self.nf + D, dtype=torch.float32, device=dev)
@@ -201,17 +265,19 @@ class TrainEngine:
         # ---- blocks, last to first (latte.py:177-181) ----
         for i in reversed(range(m.depth)):
             xs, h1, qkv, o, m1, xm, h2, u, a, m2 = S["blocks"].pop()
-            mv = mod[:, i * 6 * D:(i + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-            dv = dmod[:, i * 6 * D:(i + 1) * 6 * D]
-            dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
             temporal = bool(i % 2)
+            mv = (mod_t if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
+            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
+            dv = (dmod_t if temporal else dmod)[:, i * 6 * D:(i + 1) * 6 * D]
+            dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
+            rp = rpb_t if temporal else rpb
+            dxb = dx[:Tv] if temporal else dx   # a temporal block passes the image rows' gradient through untouched
             wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
             p = f"blocks.{i}."
             G[p + "attn.qkv.bias"], G[p + "attn.proj.bias"] = bias_view(i, 0, 3 * D), bias_view(i, 3 * D, D)
             G[p + "mlp.fc1.bias"], G[p + "mlp.fc2.bias"] = bias_view(i, 4 * D, Hm), bias_view(i, 4 * D + Hm, D)
             # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod(x_mid))))
-            dm2 = ops.gate_bwd(dx, m2, g2, rpb, dg2, G[p + "mlp.fc2.bias"])
+            dm2 = ops.gate_bwd(dxb, m2, g2, rp, dg2, G[p + "mlp.fc2.bias"])
             G[p + "mlp.fc2.weight"] = wgrad(dm2, a)
             del a
             # gelu'(u) is a separate pass: in this dgrad's epilogue it made the GEMM the bottleneck (327 us vs 153 + 129 us)
@@ -221,20 +287,20 @@ class TrainEngine:
             G[p + "mlp.fc1.weight"] = wgrad(du, h2)
             dh2 = ops.dgrad(du, w1[0])
             del du
-            ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rpb, dx, dsh2, dsc2)
+            ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rp, dxb, dsh2, dsc2)
             del dh2
             # x_mid = x_in + g1 * proj(attn(qkv(LNmod(x_in))))
-            dm1 = ops.gate_bwd(dx, m1, g1, rpb, dg1, G[p + "attn.proj.bias"])
+            dm1 = ops.gate_bwd(dxb, m1, g1, rp, dg1, G[p + "attn.proj.bias"])
             G[p + "attn.proj.weight"] = wgrad(dm1, o)
             do = ops.dgrad(dm1, wp[0])
             del dm1
-            dqkv = ops.attention_bwd(qkv, o, do, B, Fr, N, H, temporal)
+            dqkv = ops.attention_bwd(qkv, o, do, B, Fr if temporal else Fr + self.images, N, H, temporal)
             del do
             ops.colsum(dqkv, G[p + "attn.qkv.bias"])
             G[p + "attn.qkv.weight"] = wgrad(dqkv, h1)
             dh1 = ops.dgrad(dqkv, wq[0])
             del dqkv
-            ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rpb, dx, dsh1, dsc1)
+            ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rp, dxb, dsh1, dsc1)
             del dh1, xs, h1, qkv, o, m1, xm, h2, u, m2
 
         # ---- patch embedding (latte.py:330-331; pos_embed / temp_embed are frozen, :246-247) ----
@@ -294,10 +360,10 @@ class _LatteTrainFn(torch.autograd.Function):
         return (None, None, None, dc) + grads
 
 
-def train_forward(model, ops, dtype, x, c):
+def train_forward(model, ops, dtype, x, c, images=0):
     """Forward of one training step with the backward attached.  c = t_embedder(t) + y_embedder(y), computed by the caller with
-    torch autograd (a (B, D) graph)."""
-    eng = TrainEngine(model, ops, dtype)
+    torch autograd (a (B, D) graph); with `images` still frames per sample, the per-frame `frame_conditioning` instead."""
+    eng = TrainEngine(model, ops, dtype, images)
     names = trainable_names(model)
     named = dict(model.named_parameters())
     params = [named[n] for n in names]
@@ -307,12 +373,39 @@ def train_forward(model, ops, dtype, x, c):
 def conditioning(model, t, y):
     """c = t_embedder(t) [+ y_embedder(y)] with torch autograd (latte.py:98-123 sincos + MLP, :148-153 table lookup): a
     (B, D) graph of a handful of kernels whose parameters get their gradients from `dc`."""
+    c = _timestep_embedding(model, t)
+    if model.extras == 2:
+        c = c + model.y_embedder.embedding_table(y).float()
+    return c
+
+
+def _timestep_embedding(model, t):
     import math
     half = model.t_embedder.frequency_embedding_size // 2
     freqs = torch.exp(-math.log(10000) * torch.arange(0, half, dtype=torch.float32, device=t.device) / half)
     args = t[:, None].float() * freqs[None]
     emb = torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
-    c = model.t_embedder.mlp(emb.to(model.t_embedder.mlp[0].weight.dtype)).float()
+    return model.t_embedder.mlp(emb.to(model.t_embedder.mlp[0].weight.dtype)).float()
+
+
+def frame_conditioning(model, t, y, y_image, images):
+    """Per-frame conditioning of video + image joint training (latte_img.py:331, 336-349), (B*(F+I), D) in the engine's row
+    order: the B*F video frames first, (b, f) -> t_emb[b] [+ y_emb(y[b])], then the B*I images, (b, i) -> t_emb[b]
+    [+ y_emb(y_image[b, i])].  y_image (B, I) int64; labels already dropped by the caller.  Torch autograd carries `dc` back to
+    the embedders, as for `conditioning`."""
+    temb = _timestep_embedding(model, t)
+    B, D = temb.shape
+    cv, ci = temb, temb[:, None].expand(B, images, D)
     if model.extras == 2:
-        c = c + model.y_embedder.embedding_table(y).float()
-    return c
+        table = model.y_embedder.embedding_table
+        cv = cv + table(y).float()
+        ci = ci + table(y_image).float()
+    return torch.cat((cv.repeat_interleave(model.num_frames, dim=0), ci.reshape(B * images, D)))
+
+
+def image_forward(model, ops, dtype, x, c, images):
+    """Forward only (no activations kept, no autograd node) of a video + image batch through the training engine."""
+    eng = TrainEngine(model, ops, dtype, images)
+    with torch.no_grad():
+        eng.prepare()
+        return eng.forward(x.detach().float(), c.detach(), save=False)
