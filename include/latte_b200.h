@@ -436,6 +436,17 @@ B200_API int b200_ln_modulate_bwd(const void* dh16, const float* x, const float*
  * temporal sequences of 16 frames or fewer).                                                                                */
 B200_API int b200_attention_bwd(const void* qkv16, const void* o16, const void* do16, void* dqkv16, float* stats, int batch,
                                 int frames, int tokens, int heads, int head_dim, int dtype, int temporal, void* stream);
+/* backward of b200_cross_attention (default scale, no key/value padding rows): dq16 [batch*q_rows_per_batch, heads*head_dim]
+ * and dK / dV written into dkv16 [batch*kv_len, dkv_row_stride] at columns [dkv_col0, dkv_col0 + 2*heads*head_dim) in the kv
+ * operand's own order [k heads | v heads]; the other columns are not touched.  q, kv, key_bias as in b200_cross_attention; o16
+ * its output, do16 the output's gradient.  head_dim 64 or 72 (others return B200_ERR_UNSUPPORTED), kv_len 1..128,
+ * q_rows_per_batch % 128 == 0.  dK / dV sum a fixed number of per-chunk fp32 partials in a fixed order: bit-reproducible.
+ * workspace: >= b200_cross_attention_bwd_workspace_bytes(...) bytes, 16-byte aligned (0 = unsupported shape).             */
+B200_API size_t b200_cross_attention_bwd_workspace_bytes(int batch, int q_rows_per_batch, int kv_len, int heads, int head_dim);
+B200_API int b200_cross_attention_bwd(const void* q, const void* kv, const float* key_bias, const void* o16, const void* do16, void* dq16,
+                                      void* dkv16, int dkv_row_stride, int dkv_col0, int batch, int q_rows_per_batch, int kv_len,
+                                      int q_row_stride, int kv_row_stride, int heads, int head_dim, int dtype, void* workspace,
+                                      size_t workspace_bytes, void* stream);
 /* adaLN_modulation Linear on `batch` <= 8 conditioning rows (all blocks stacked, NA = depth*6*dim + 2*dim output features):
  * dW[NA, dim] (fp32, overwritten) = dmod^T . sc16;  dsc[batch, dim] (fp32, overwritten) = dmod . W16.                     */
 B200_API int b200_ada_outer(const float* dmod, int64_t dmod_batch_stride, const void* sc16, float* dW, int batch, int NA, int dim,

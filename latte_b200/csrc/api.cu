@@ -745,6 +745,24 @@ B200_API int b200_attention_bwd(const void* qkv16, const void* o16, const void* 
   return b200::launch_attention_bwd(qkv16, o16, do16, dqkv16, stats, batch, frames, tokens, heads, head_dim, dtype == B200_BF16,
                                     temporal, static_cast<cudaStream_t>(stream));
 }
+B200_API size_t b200_cross_attention_bwd_workspace_bytes(int batch, int q_rows_per_batch, int kv_len, int heads, int head_dim) {
+  return b200::cross_attention_bwd_workspace_bytes(batch, q_rows_per_batch, kv_len, heads, head_dim);
+}
+B200_API int b200_cross_attention_bwd(const void* q, const void* kv, const float* key_bias, const void* o16, const void* do16, void* dq16,
+                                      void* dkv16, int dkv_row_stride, int dkv_col0, int batch, int q_rows_per_batch, int kv_len,
+                                      int q_row_stride, int kv_row_stride, int heads, int head_dim, int dtype, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  B200_DT(dtype);
+  B200_TRY(b200::check_arch());
+  b200::CrossAttnBwdArgs a{};
+  a.q = q; a.kv = kv; a.key_bias = key_bias; a.o = o16; a.d_o = do16; a.dq = dq16; a.dkv = dkv16;
+  a.dkv_row_stride = dkv_row_stride; a.dkv_col0 = dkv_col0;
+  a.batch = batch; a.q_rows_per_batch = q_rows_per_batch; a.kv_len = kv_len;
+  a.q_row_stride = q_row_stride; a.kv_row_stride = kv_row_stride; a.heads = heads; a.head_dim = head_dim;
+  a.bf16 = dtype == B200_BF16;
+  a.workspace = workspace; a.workspace_bytes = workspace_bytes;
+  return b200::launch_cross_attention_bwd(a, static_cast<cudaStream_t>(stream));
+}
 B200_API int b200_ada_outer(const float* dmod, int64_t dmod_batch_stride, const void* sc16, float* dW, int batch, int NA, int dim,
                             int dtype, void* stream) {
   B200_DT(dtype);

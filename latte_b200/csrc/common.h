@@ -181,6 +181,25 @@ int launch_ln_modulate_bwd(const void* dh16, const float* x, const float* scale,
                            float* dshift, float* dscale, long long dmod_bs, int rows, int dim, int bf16, cudaStream_t stream);
 int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* dqkv, float* stats, int batch, int frames, int tokens,
                          int heads, int head_dim, int bf16, int temporal, cudaStream_t stream);
+// backward of launch_cross_attention (no pos_bias, default scale, kv_batch_rows = kv_len)
+struct CrossAttnBwdArgs {
+  const void* q;          // as CrossAttnArgs
+  const void* kv;
+  const float* key_bias;
+  const void* o;          // the forward's output [batch * q_rows_per_batch, heads*head_dim] 16-bit
+  const void* d_o;        // its gradient, same layout
+  void* dq;               // [batch * q_rows_per_batch, heads*head_dim] 16-bit
+  void* dkv;              // [batch * kv_len, dkv_row_stride] 16-bit; columns [dkv_col0, dkv_col0 + 2*heads*head_dim) are written
+  int dkv_row_stride, dkv_col0;
+  int batch, q_rows_per_batch, kv_len;
+  int q_row_stride, kv_row_stride;
+  int heads, head_dim;
+  int bf16;
+  void* workspace;
+  size_t workspace_bytes;
+};
+size_t cross_attention_bwd_workspace_bytes(int batch, int q_rows_per_batch, int kv_len, int heads, int head_dim);
+int launch_cross_attention_bwd(const CrossAttnBwdArgs& a, cudaStream_t stream);
 int launch_ada_outer(const float* dmod, long long dmod_bs, const void* sc16, float* dW, int batch, int NA, int dim, int bf16, cudaStream_t stream);
 int launch_ada_dsc(const float* dmod, long long dmod_bs, const void* w16, float* dsc, int batch, int NA, int dim, int bf16, cudaStream_t stream);
 

@@ -826,6 +826,244 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const uint16_t* __res
   }
 }
 
+// ------------------------------------------------------------------------------------------------ cross-attention backward
+// Backward of b200_cross_attention, softmax(q k^T hd^-1/2 + key_bias) v, on the tile code above.  All kv_len <= 128 keys of a
+// sample sit in one or two 64-row tiles; rows at or beyond kv_len are zero-filled and their scores are -inf, so P = 0 exactly
+// there.  The key bias (-10000 for a masked prompt token) is added in fp32 exactly as the forward adds it.  The softmax scale is
+// applied to the fp32 dQ / dK accumulators, never to the 16-bit dS (see kernel A above).
+//   xattn_bwd_dq:     one CTA = 64 query rows of one (sample, head): row statistics from q and k, delta = rowsum(dO.O), dQ = dS K;
+//                     writes dQ and the statistics.
+//   xattn_bwd_dkv:    one CTA = one of `chunks` contiguous ranges of a sample's query blocks, one head, every key (one warp per 16
+//                     keys): an fp32 [dK | dV] partial per chunk.
+//   xattn_bwd_reduce: sums the partials in chunk order and writes 16-bit dK / dV.  No atomics: reruns are bit-identical.
+struct XAttnBwd {
+  const uint16_t* q;        // [batch*q_rows, q_ld]
+  const uint16_t* kv;       // [batch*kv_len, kv_ld], columns [k heads | v heads]
+  const float* key_bias;    // [batch, 128] or nullptr
+  const uint16_t* o;        // [batch*q_rows, heads*HD]
+  const uint16_t* d_o;
+  uint16_t* dq;             // [batch*q_rows, heads*HD]
+  float* lse;               // [batch][heads][q_rows], log2 units
+  float* delta;
+  float* part;              // [batch][heads][chunks][128][2*HD]
+  int q_rows, kv_len, q_ld, kv_ld, heads, chunks;
+  float scale_log2;
+};
+
+constexpr float kXLog2e = 1.4426950408889634f;
+
+// scores of a warp's [16 queries x 64 keys] block kt in log2 units with the key bias, -inf at keys >= kv_len
+__device__ __forceinline__ void xattn_scores(float (&acc)[8][4], const float* sB, int kt, int kv_len, float scale_log2) {
+  const int c0 = kt * 64 + (threadIdx.x & 3) * 2;
+#pragma unroll
+  for (int n = 0; n < 8; ++n)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = c0 + n * 8 + (e & 1);
+      acc[n][e] = c < kv_len ? fmaf(sB[c], kXLog2e, acc[n][e] * scale_log2) : -INFINITY;
+    }
+}
+
+template <bool BF16, int HD>
+__global__ void __launch_bounds__(128) xattn_bwd_dq_kernel(const XAttnBwd p) {
+  using G = AB<HD>;
+  extern __shared__ __align__(16) uint16_t sm[];
+  uint16_t* sQ = sm;
+  uint16_t* sDO = sm + G::TILE;
+  uint16_t* sO = sm + 2 * G::TILE;
+  uint16_t* sK = sm + 3 * G::TILE;      // 2 tiles = keys 0..127
+  uint16_t* sV = sm + 5 * G::TILE;      // 2 tiles
+  float* sB = reinterpret_cast<float*>(sm + 7 * G::TILE);    // [128] key bias
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int D = p.heads * HD;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const size_t qrow0 = static_cast<size_t>(b) * p.q_rows + qb * 64;
+  const size_t krow0 = static_cast<size_t>(b) * p.kv_len;
+  const int nkt = (p.kv_len + 63) / 64;
+  zero_pads<HD>(sm, 7);
+  load_tile64<HD>(sQ, p.q, qrow0, p.q_ld, h * HD);
+  load_tile64<HD>(sDO, p.d_o, qrow0, D, h * HD);
+  load_tile64<HD>(sO, p.o, qrow0, D, h * HD);
+  for (int kt = 0; kt < nkt; ++kt) {
+    load_tile64<HD, true>(sK + kt * G::TILE, p.kv, krow0 + kt * 64, p.kv_ld, h * HD, 1, p.kv_len - kt * 64);
+    load_tile64<HD, true>(sV + kt * G::TILE, p.kv, krow0 + kt * 64, p.kv_ld, D + h * HD, 1, p.kv_len - kt * 64);
+  }
+  for (int c = threadIdx.x; c < 128; c += blockDim.x) sB[c] = p.key_bias && c < p.kv_len ? p.key_bias[b * 128 + c] : 0.f;
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();
+  const int r_lo = warp * 16 + (lane >> 2);
+  float dl[2] = {0.f, 0.f};
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int r = r_lo + hh * 8;
+    for (int c = (lane & 3) * 2; c < HD; c += 8) {
+      const float2 a = unpack2<BF16>(*reinterpret_cast<const uint32_t*>(sDO + r * G::HDP + c));
+      const float2 v = unpack2<BF16>(*reinterpret_cast<const uint32_t*>(sO + r * G::HDP + c));
+      dl[hh] += a.x * v.x + a.y * v.y;
+    }
+    dl[hh] += __shfl_xor_sync(0xffffffffu, dl[hh], 1);
+    dl[hh] += __shfl_xor_sync(0xffffffffu, dl[hh], 2);
+  }
+  // ---- pass 1: row max / sum over the sample's keys
+  float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
+  for (int kt = 0; kt < nkt; ++kt) {
+    float acc[8][4] = {};
+    mm_a_tileT<BF16, HD>(acc, sQ, warp * 16, sK + kt * G::TILE);
+    xattn_scores(acc, sB, kt, p.kv_len, p.scale_log2);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float m = mx[hh];
+#pragma unroll
+      for (int n = 0; n < 8; ++n) m = fmaxf(m, fmaxf(acc[n][2 * hh], acc[n][2 * hh + 1]));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+      float sacc = 0.f;
+#pragma unroll
+      for (int n = 0; n < 8; ++n) sacc += exp2f(acc[n][2 * hh] - m) + exp2f(acc[n][2 * hh + 1] - m);
+      sum[hh] = sum[hh] * exp2f(mx[hh] - m) + sacc;
+      mx[hh] = m;
+    }
+  }
+  float l2[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float t = sum[hh];
+    t += __shfl_xor_sync(0xffffffffu, t, 1);
+    t += __shfl_xor_sync(0xffffffffu, t, 2);
+    l2[hh] = mx[hh] + log2f(t);
+    if ((lane & 3) == 0) {
+      const size_t idx = (static_cast<size_t>(b) * p.heads + h) * p.q_rows + qb * 64 + r_lo + hh * 8;
+      p.lse[idx] = l2[hh];
+      p.delta[idx] = dl[hh];
+    }
+  }
+  // ---- pass 2: dS = P (dP - delta), dQ = dS K
+  float dq[G::NT][4] = {};
+  for (int kt = 0; kt < nkt; ++kt) {
+    const uint16_t* cK = sK + kt * G::TILE;
+    float s_acc[8][4] = {}, p_acc[8][4] = {};
+    mm_a_tileT<BF16, HD>(s_acc, sQ, warp * 16, cK);
+    mm_a_tileT<BF16, HD>(p_acc, sDO, warp * 16, sV + kt * G::TILE);
+    xattn_scores(s_acc, sB, kt, p.kv_len, p.scale_log2);
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hh = e >> 1;
+        s_acc[n][e] = exp2f(s_acc[n][e] - l2[hh]) * (p_acc[n][e] - dl[hh]);
+      }
+    uint32_t pds[4][4];
+    acc_to_afrag<BF16>(pds, s_acc);
+    mm_p_tile<BF16, HD>(dq, pds, cK);
+  }
+  const float sc = p.scale_log2 * 0.6931471805599453f;
+#pragma unroll
+  for (int n = 0; n < G::NT; ++n)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) dq[n][e] *= sc;
+  store_rows<BF16, HD>(p.dq, qrow0, D, h * HD, dq, warp * 16, 64);
+}
+
+// launched with (kv_len + 63) / 64 * 128 threads: warp w owns keys [16w, 16w + 16)
+template <bool BF16, int HD>
+__global__ void __launch_bounds__(256) xattn_bwd_dkv_kernel(const XAttnBwd p) {
+  using G = AB<HD>;
+  extern __shared__ __align__(16) uint16_t sm[];
+  uint16_t* sK = sm;                    // 2 tiles
+  uint16_t* sV = sm + 2 * G::TILE;      // 2 tiles
+  uint16_t* sQ = sm + 4 * G::TILE;      // [2] buffers
+  uint16_t* sDO = sm + 6 * G::TILE;     // [2] buffers
+  float* sL = reinterpret_cast<float*>(sm + 8 * G::TILE);   // [2][64] lse, then [2][64] delta
+  float* sD = sL + 128;
+  const int chunk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int D = p.heads * HD;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const size_t qrow0 = static_cast<size_t>(b) * p.q_rows;
+  const size_t krow0 = static_cast<size_t>(b) * p.kv_len;
+  const size_t stat0 = (static_cast<size_t>(b) * p.heads + h) * p.q_rows;
+  const int nqb = p.q_rows / 64, nkt = (p.kv_len + 63) / 64;
+  const int qb0 = chunk * nqb / p.chunks, qb1 = (chunk + 1) * nqb / p.chunks;
+  auto load_q = [&](int qb, int buf) {
+    load_tile64<HD>(sQ + buf * G::TILE, p.q, qrow0 + qb * 64, p.q_ld, h * HD);
+    load_tile64<HD>(sDO + buf * G::TILE, p.d_o, qrow0 + qb * 64, D, h * HD);
+    if (threadIdx.x < 16) cp_async16(sL + buf * 64 + threadIdx.x * 4, p.lse + stat0 + qb * 64 + threadIdx.x * 4);
+    else if (threadIdx.x < 32) cp_async16(sD + buf * 64 + (threadIdx.x - 16) * 4, p.delta + stat0 + qb * 64 + (threadIdx.x - 16) * 4);
+  };
+  zero_pads<HD>(sm, 8);
+  for (int kt = 0; kt < nkt; ++kt) {
+    load_tile64<HD, true>(sK + kt * G::TILE, p.kv, krow0 + kt * 64, p.kv_ld, h * HD, 1, p.kv_len - kt * 64);
+    load_tile64<HD, true>(sV + kt * G::TILE, p.kv, krow0 + kt * 64, p.kv_ld, D + h * HD, 1, p.kv_len - kt * 64);
+  }
+  load_q(qb0, 0);
+  cp_async_commit();
+  // the two keys of this thread's accumulator rows: validity and bias
+  bool kvalid[2];
+  float kbias[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int k = warp * 16 + (lane >> 2) + hh * 8;
+    kvalid[hh] = k < p.kv_len;
+    kbias[hh] = p.key_bias && kvalid[hh] ? p.key_bias[b * 128 + k] : 0.f;
+  }
+  cp_async_wait<0>();
+  __syncthreads();
+  float dk[G::NT][4] = {}, dv[G::NT][4] = {};
+  for (int qb = qb0; qb < qb1; ++qb) {
+    const int cur = (qb - qb0) & 1;
+    if (qb + 1 < qb1) load_q(qb + 1, cur ^ 1);
+    cp_async_commit();
+    const uint16_t* cQ = sQ + cur * G::TILE;
+    const uint16_t* cDO = sDO + cur * G::TILE;
+    const float* cL = sL + cur * 64;
+    const float* cD = sD + cur * 64;
+    float s_acc[8][4] = {}, p_acc[8][4] = {};
+    mm_a_tileT<BF16, HD>(s_acc, sK, warp * 16, cQ);      // [16 keys x 64 queries]
+    mm_a_tileT<BF16, HD>(p_acc, sV, warp * 16, cDO);
+    uint32_t pp[4][4], pds[4][4];
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hh = e >> 1, qi = n * 8 + (lane & 3) * 2 + (e & 1);
+        const float pr = kvalid[hh] ? exp2f(fmaf(kbias[hh], kXLog2e, s_acc[n][e] * p.scale_log2) - cL[qi]) : 0.f;
+        p_acc[n][e] = pr * (p_acc[n][e] - cD[qi]);
+        s_acc[n][e] = pr;
+      }
+    acc_to_afrag<BF16>(pp, s_acc);
+    acc_to_afrag<BF16>(pds, p_acc);
+    mm_p_tile<BF16, HD>(dv, pp, cDO);
+    mm_p_tile<BF16, HD>(dk, pds, cQ);
+    cp_async_wait<0>();
+    __syncthreads();
+  }
+  const float sc = p.scale_log2 * 0.6931471805599453f;
+  float* dst = p.part + ((static_cast<size_t>(b) * p.heads + h) * p.chunks + chunk) * 128 * (2 * HD);
+  const int r = warp * 16 + (lane >> 2);
+#pragma unroll
+  for (int n = 0; n < G::NT; ++n) {
+    const int c = n * 8 + (lane & 3) * 2;
+    *reinterpret_cast<float2*>(dst + r * (2 * HD) + c) = make_float2(dk[n][0] * sc, dk[n][1] * sc);
+    *reinterpret_cast<float2*>(dst + (r + 8) * (2 * HD) + c) = make_float2(dk[n][2] * sc, dk[n][3] * sc);
+    *reinterpret_cast<float2*>(dst + r * (2 * HD) + HD + c) = make_float2(dv[n][0], dv[n][1]);
+    *reinterpret_cast<float2*>(dst + (r + 8) * (2 * HD) + HD + c) = make_float2(dv[n][2], dv[n][3]);
+  }
+}
+
+// dkv[(b*kv_len + j) * ld + col0 + col] = sum over chunks (in order) of the partials; col in [0, 2D): [k heads | v heads]
+template <bool BF16>
+__global__ void __launch_bounds__(256) xattn_bwd_reduce_kernel(const float* __restrict__ part, uint16_t* __restrict__ dkv, int ld,
+                                                               int col0, int kv_len, int heads, int hd, int chunks) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y, b = blockIdx.z;
+  const int D = heads * hd;
+  if (col >= 2 * D) return;
+  const int kind = col >= D, hh = (col - kind * D) / hd, d = col - kind * D - hh * hd;
+  const float* src = part + ((static_cast<size_t>(b) * heads + hh) * chunks * 128 + j) * (2 * hd) + kind * hd + d;
+  float s = 0.f;
+  for (int c = 0; c < chunks; ++c) s += src[static_cast<size_t>(c) * 128 * (2 * hd)];
+  dkv[(static_cast<size_t>(b) * kv_len + j) * ld + col0 + col] = rnd1<BF16>(s);
+}
+
 // ------------------------------------------------------------------------------------------------ attention backward (temporal)
 // Sequences of F <= 16 frames at a fixed token: rows (b, f, n), f = 0..F-1 (row stride `tokens`), head_dim 64 / 72, on tensor
 // cores.  ONE WARP per (b, n, head), four heads per CTA, no block-level synchronisation.  The F <= 16 frames of q, k, v, dO
@@ -1270,6 +1508,92 @@ int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* 
   }
   if (bf16) return attn_bwd_two_pass<true, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
   return attn_bwd_two_pass<false, 64>(q, oo, g, dq, lse, delta, nseq, tokens, heads, stream);
+}
+
+// Query chunks per (sample, head) of the dK/dV reduction: at least 4 query blocks (256 rows) per chunk, at most 16 chunks.  A
+// function of the shape alone, so the summation order never changes between runs.
+static int xattn_chunks(int q_rows_per_batch) {
+  const int c = q_rows_per_batch / 64 / 4;
+  return c < 1 ? 1 : (c > 16 ? 16 : c);
+}
+
+static int xattn_bwd_check(int batch, int q_rows_per_batch, int kv_len, int heads, int head_dim) {
+  B200_REQUIRE(batch > 0 && q_rows_per_batch > 0 && heads > 0, B200_ERR_SHAPE, "cross_attention_bwd: bad shape");
+  B200_REQUIRE(head_dim == 64 || head_dim == 72, B200_ERR_UNSUPPORTED, "cross_attention_bwd: head_dim %d not built (64, 72)", head_dim);
+  B200_REQUIRE(kv_len >= 1 && kv_len <= 128, B200_ERR_UNSUPPORTED, "cross_attention_bwd: %d keys per sample (1..128 built)", kv_len);
+  B200_REQUIRE(q_rows_per_batch % 128 == 0, B200_ERR_UNSUPPORTED,
+               "cross_attention_bwd: query rows per sample %d must be a multiple of 128", q_rows_per_batch);
+  B200_REQUIRE(batch <= 65535 && heads <= 65535, B200_ERR_UNSUPPORTED, "cross_attention_bwd: batch / heads exceed the grid");
+  return B200_OK;
+}
+
+static size_t xattn_stats_bytes(int batch, int q_rows_per_batch, int heads) {
+  return (static_cast<size_t>(2) * batch * heads * q_rows_per_batch * sizeof(float) + 255) / 256 * 256;
+}
+
+size_t cross_attention_bwd_workspace_bytes(int batch, int q_rows_per_batch, int kv_len, int heads, int head_dim) {
+  if (xattn_bwd_check(batch, q_rows_per_batch, kv_len, heads, head_dim) != B200_OK) return 0;
+  const size_t part = static_cast<size_t>(batch) * heads * xattn_chunks(q_rows_per_batch) * 128 * 2 * head_dim * sizeof(float);
+  return xattn_stats_bytes(batch, q_rows_per_batch, heads) + part;
+}
+
+template <bool BF16, int HD>
+static int xattn_bwd_launch(const XAttnBwd& p, int batch, uint16_t* dkv, int dkv_ld, int dkv_col0, cudaStream_t stream) {
+  using G = AB<HD>;
+  auto ka = xattn_bwd_dq_kernel<BF16, HD>;
+  auto kb = xattn_bwd_dkv_kernel<BF16, HD>;
+  const size_t smem_a = static_cast<size_t>(7) * G::TILE * 2 + 128 * sizeof(float);
+  const size_t smem_b = static_cast<size_t>(8) * G::TILE * 2 + 256 * sizeof(float);
+  B200_SET_SMEM_ONCE(ka, static_cast<int>(smem_a));
+  B200_SET_SMEM_ONCE(kb, static_cast<int>(smem_b));
+  ka<<<dim3(p.q_rows / 64, p.heads, batch), 128, smem_a, stream>>>(p);
+  B200_CHECK_CUDA(cudaGetLastError());
+  kb<<<dim3(p.chunks, p.heads, batch), (p.kv_len + 63) / 64 * 128, smem_b, stream>>>(p);
+  B200_CHECK_CUDA(cudaGetLastError());
+  const int D2 = 2 * p.heads * HD;
+  xattn_bwd_reduce_kernel<BF16><<<dim3((D2 + 255) / 256, p.kv_len, batch), 256, 0, stream>>>(p.part, dkv, dkv_ld, dkv_col0, p.kv_len,
+                                                                                           p.heads, HD, p.chunks);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return B200_OK;
+}
+
+int launch_cross_attention_bwd(const CrossAttnBwdArgs& a, cudaStream_t stream) {
+  B200_TRY(xattn_bwd_check(a.batch, a.q_rows_per_batch, a.kv_len, a.heads, a.head_dim));
+  const int D = a.heads * a.head_dim;
+  B200_REQUIRE(a.q_row_stride >= D && a.kv_row_stride >= 2 * D && a.q_row_stride % 8 == 0 && a.kv_row_stride % 8 == 0, B200_ERR_SHAPE,
+               "cross_attention_bwd: bad q / kv row strides");
+  B200_REQUIRE(a.dkv_col0 >= 0 && a.dkv_row_stride >= a.dkv_col0 + 2 * D, B200_ERR_SHAPE, "cross_attention_bwd: bad dkv column window");
+  B200_REQUIRE(ALIGNED16(a.q) && ALIGNED16(a.kv) && ALIGNED16(a.o) && ALIGNED16(a.d_o) && ALIGNED16(a.dq) && ALIGNED16(a.workspace),
+               B200_ERR_ALIGN, "cross_attention_bwd: q / kv / o / do / dq / workspace must be 16-byte aligned");
+  B200_REQUIRE(a.dkv != nullptr, B200_ERR_SHAPE, "cross_attention_bwd: dkv missing");
+  const size_t need = cross_attention_bwd_workspace_bytes(a.batch, a.q_rows_per_batch, a.kv_len, a.heads, a.head_dim);
+  B200_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= need, B200_ERR_WORKSPACE,
+               "cross_attention_bwd: workspace too small: need %zu bytes, got %zu", need, a.workspace_bytes);
+  XAttnBwd p{};
+  p.q = static_cast<const uint16_t*>(a.q);
+  p.kv = static_cast<const uint16_t*>(a.kv);
+  p.key_bias = a.key_bias;
+  p.o = static_cast<const uint16_t*>(a.o);
+  p.d_o = static_cast<const uint16_t*>(a.d_o);
+  p.dq = static_cast<uint16_t*>(a.dq);
+  const size_t nstat = static_cast<size_t>(a.batch) * a.heads * a.q_rows_per_batch;
+  p.lse = static_cast<float*>(a.workspace);
+  p.delta = p.lse + nstat;
+  p.part = reinterpret_cast<float*>(static_cast<uint8_t*>(a.workspace) + xattn_stats_bytes(a.batch, a.q_rows_per_batch, a.heads));
+  p.q_rows = a.q_rows_per_batch;
+  p.kv_len = a.kv_len;
+  p.q_ld = a.q_row_stride;
+  p.kv_ld = a.kv_row_stride;
+  p.heads = a.heads;
+  p.chunks = xattn_chunks(a.q_rows_per_batch);
+  p.scale_log2 = kXLog2e / sqrtf(static_cast<float>(a.head_dim));
+  uint16_t* dkv = static_cast<uint16_t*>(a.dkv);
+  if (a.head_dim == 72) {
+    if (a.bf16) return xattn_bwd_launch<true, 72>(p, a.batch, dkv, a.dkv_row_stride, a.dkv_col0, stream);
+    return xattn_bwd_launch<false, 72>(p, a.batch, dkv, a.dkv_row_stride, a.dkv_col0, stream);
+  }
+  if (a.bf16) return xattn_bwd_launch<true, 64>(p, a.batch, dkv, a.dkv_row_stride, a.dkv_col0, stream);
+  return xattn_bwd_launch<false, 64>(p, a.batch, dkv, a.dkv_row_stride, a.dkv_col0, stream);
 }
 
 int launch_ada_outer(const float* dmod, long long dmod_bs, const void* sc16, float* dW, int batch, int NA, int dim, int bf16, cudaStream_t stream) {

@@ -149,6 +149,39 @@ class NativeOps:
         _lib.check(rc, "b200_attention_bwd")
         return dqkv
 
+    def cross_attention(self, q, kv, B, q_rows, L, H, key_bias=None):
+        """Text cross-attention (b200_cross_attention): q [B*q_rows, H*hd]; kv a row-major view [>= B*L, 2*H*hd] ([k | v]
+        heads, any row stride: a column window of the stacked K/V of all layers); key_bias None or fp32 [B, 128]."""
+        self._cuda(q, kv, key_bias)
+        assert q.is_contiguous() and kv.stride(1) == 1 and q.dtype == kv.dtype == self.dtype
+        D = q.shape[1]
+        out = torch.empty_like(q)
+        with torch.cuda.device(q.device):
+            rc = _lib.load().b200_cross_attention(q.data_ptr(), kv.data_ptr(), key_bias.data_ptr() if key_bias is not None else None,
+                                                  out.data_ptr(), B, q_rows, L, q.stride(0), kv.stride(0), H, D // H, self.dt, _s(q))
+        _lib.check(rc, "b200_cross_attention")
+        return out
+
+    def cross_attention_bwd(self, q, kv, o, do, B, q_rows, L, H, key_bias, dkv, col0):
+        """Backward of `cross_attention`: returns dq; dK | dV go to dkv[:B*L, col0:col0 + 2*H*hd] (dkv 16-bit, row-major)."""
+        self._cuda(q, kv, o, do, key_bias, dkv)
+        assert q.is_contiguous() and o.is_contiguous() and do.is_contiguous() and kv.stride(1) == 1 and dkv.stride(1) == 1
+        D = q.shape[1]
+        lib = _lib.load()
+        need = lib.b200_cross_attention_bwd_workspace_bytes(B, q_rows, L, H, D // H)
+        if need == 0:
+            raise RuntimeError("b200_cross_attention_bwd: unsupported shape: " + _lib.last_error())
+        ws = getattr(self, "_xattn_ws", None)
+        if ws is None or ws.numel() < need or ws.device != q.device:   # reused by every layer, in stream order
+            ws = self._xattn_ws = torch.empty(need, dtype=torch.uint8, device=q.device)
+        dq = torch.empty_like(q)
+        with torch.cuda.device(q.device):
+            rc = lib.b200_cross_attention_bwd(q.data_ptr(), kv.data_ptr(), key_bias.data_ptr() if key_bias is not None else None,
+                                              o.data_ptr(), do.data_ptr(), dq.data_ptr(), dkv.data_ptr(), dkv.stride(0), col0, B, q_rows,
+                                              L, q.stride(0), kv.stride(0), H, D // H, self.dt, ws.data_ptr(), ws.numel(), _s(q))
+        _lib.check(rc, "b200_cross_attention_bwd")
+        return dq
+
     def colsum(self, a, out):
         self._cuda(a, out)
         assert a.is_contiguous() and out.is_contiguous() and out.dtype == torch.float32
