@@ -24,6 +24,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._cache import DeviceCacheMixin
+from .training import GradientCheckpointingMixin
 
 
 # ------------------------------------------------------------------------------------------------
@@ -106,7 +107,7 @@ def _sincos_2d(dim: int, grid: int) -> np.ndarray:
     return np.concatenate([_sincos_1d(dim // 2, ww), _sincos_1d(dim // 2, hh)], axis=1)
 
 
-class Latte(DeviceCacheMixin, nn.Module):
+class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
     """Diffusion transformer with alternating spatial / temporal blocks (reference latte.py:204-398)."""
 
     def __init__(self, input_size=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
@@ -156,6 +157,8 @@ class Latte(DeviceCacheMixin, nn.Module):
         #: eval-mode calls replay a CUDA graph of the whole forward (captured per (batch, cfg) signature on its second
         #: use; results are bit-identical to the eager launch sequence).  Set False to always launch eagerly.
         self.use_cuda_graphs = True
+        #: training steps keep each block's input only and rerun the block in the backward (`enable_gradient_checkpointing`)
+        self.gradient_checkpointing = False
 
     # -------------------------------------------------------------------------------------------
     def initialize_weights(self):

@@ -11,6 +11,10 @@ Derivatives follow the reference forward (models/latte.py): block :177-181, modu
 spatial AND temporal blocks (the regrouping of :355/:368 is index arithmetic inside the attention kernels), so every
 per-sample adaLN vector addresses `rows_per_batch = F*N` consecutive rows.
 
+Gradient checkpointing (`checkpoint=True`, the module's `gradient_checkpointing` flag): the forward keeps each block's input
+only, and the backward reruns that block's forward right before its backward.  Both steps run the same `_block_forward` /
+`_block_backward`; only the loops around them differ.
+
 `TrainEngine` is backend-agnostic: the product backend is latte_b200.train_ops.NativeOps (C ABI, CUDA only, raises without
 the extension); tests drive the same orchestration through oracle/train_ops_oracle.TorchOps on the CPU and compare with
 gradients produced by the unmodified reference (tests/golden/train_tiny64.npz).
@@ -20,6 +24,26 @@ from __future__ import annotations
 import torch
 
 _BLOCK_LINEARS = ("attn.qkv", "attn.proj", "mlp.fc1", "mlp.fc2")
+
+
+class GradientCheckpointingMixin:
+    """Gradient checkpointing under the names of diffusers' ModelMixin (the reference LatteT2V inherits them, and
+    train_with_img.py:120-122 calls `enable_gradient_checkpointing()` when its config asks for it).  With the flag set, a
+    training step keeps only each block's input and reruns the block's forward in the backward: the saved activations shrink
+    from roughly 40-46 bytes per token and channel per block to 4, at the cost of one more forward through the blocks.  It
+    changes no result, and no call other than the training step."""
+    _supports_gradient_checkpointing = True
+    gradient_checkpointing = False
+
+    def enable_gradient_checkpointing(self):
+        self.gradient_checkpointing = True
+
+    def disable_gradient_checkpointing(self):
+        self.gradient_checkpointing = False
+
+    @property
+    def is_gradient_checkpointing(self):
+        return self.gradient_checkpointing
 
 
 def _patch_rows(x, p):
@@ -36,11 +60,13 @@ class TrainEngine:
     blocks run on the prefix x[:T_v] -- exactly a Latte batch of B videos -- with one adaLN row per video (a strided view of the
     per-frame rows), and carry the image rows through unchanged."""
 
-    def __init__(self, model, ops, dtype, images=0):
+    def __init__(self, model, ops, dtype, images=0, checkpoint=False):
         self.m = model
         self.ops = ops
         self.dtype = dtype
         self.images = images
+        #: gradient checkpointing: the forward keeps each block's input only and the backward reruns the block before its backward
+        self.checkpoint = checkpoint
         self.saved = None
         self.w = None
 
@@ -158,21 +184,110 @@ class TrainEngine:
         input's, copied device to device (B*I*N*D*4 bytes)."""
         return torch.cat((video, images))
 
+    def _block_forward(self, i, xs, mod, B, temp, rerun=False):
+        """Block i (latte.py:177-181) on its input xs (T x D fp32) -> (its output, the list of activations its backward reads).
+        rerun=True is the checkpointed backward's recomputation: it stops before the last residual update, whose output the
+        backward does not read, and returns None in its place."""
+        m, ops, W = self.m, self.ops, self.w
+        D, Fr, N, H = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads
+        _, Tv, rpb, rpb_t = self._geometry(B)
+        mod_t = self._temporal_rows(mod, B)
+        temporal = bool(i % 2)
+        mv = (mod_t if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
+        sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
+        wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
+        rp = rpb_t if temporal else rpb
+        xi = xs[:Tv] if temporal else xs        # temporal blocks see the video rows only (latte_img.py:373-374, 387-388)
+        h1 = ops.ln_modulate(xi, sh1, sc1, rp)
+        qkv = ops.linear(h1, wq[0], wq[1])
+        o = ops.attention(qkv, B, Fr if temporal else Fr + self.images, N, H, temporal)
+        m1 = ops.linear(o, wp[0], wp[1])
+        # two passes: a kernel fusing the residual update with this LayerNorm-modulate measured slower (101 vs 45 + 40 us)
+        xm = ops.gate_residual(xi, m1, g1, rp)
+        h2 = ops.ln_modulate(xm, sh2, sc2, rp)
+        u, a = ops.linear_gelu_both(h2, w1[0], w1[1])
+        m2 = ops.linear(a, w2[0], w2[1])
+        acts = [xi, h1, qkv, o, m1, xm, h2, u, a, m2]
+        if rerun:
+            return None, acts
+        if i == 0 and self.images:
+            # temp_embed goes to the video rows only (latte_img.py:377-378).  All frames of a video share one gate row, so
+            # the video rows take the per-video view, like a temporal block.
+            g2v = mod_t[:, 5 * D:6 * D]
+            xo = self._join_rows(ops.gate_residual(xm[:Tv], m2[:Tv], g2v, rpb_t, row_add=temp, tokens=N),
+                                 ops.gate_residual(xm[Tv:], m2[Tv:], g2[B * Fr:], rp))
+        else:
+            xo = ops.gate_residual(xm, m2, g2, rp, row_add=temp if i == 0 else None, tokens=N)
+            if temporal and self.images:        # image rows pass through the temporal block unchanged
+                xo = self._join_rows(xo, xs[Tv:])
+        return xo, acts
+
+    def _block_backward(self, i, acts, dx, mod, dmod, B, G, bias_flat):
+        """Backward of block i from the list `_block_forward` returned, which it empties so that each buffer is freed as soon
+        as it is used.  Accumulates into dx (T x D fp32; a temporal block touches the video rows only), dmod and the bias
+        gradients in bias_flat; puts the weight gradients and bias views into G."""
+        m, ops, W = self.m, self.ops, self.w
+        D, Fr, N, H, Hm = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads, m.mlp_hidden
+        _, Tv, rpb, rpb_t = self._geometry(B)
+        xs, h1, qkv, o, m1, xm, h2, u, a, m2 = acts
+        acts.clear()
+        temporal = bool(i % 2)
+        mv = (self._temporal_rows(mod, B) if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
+        sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
+        dv = (self._temporal_rows(dmod, B) if temporal else dmod)[:, i * 6 * D:(i + 1) * 6 * D]
+        dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
+        rp = rpb_t if temporal else rpb
+        dxb = dx[:Tv] if temporal else dx       # a temporal block passes the image rows' gradient through untouched
+        wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
+        p = f"blocks.{i}."
+        off = i * (3 * D + D + Hm + D)
+        G[p + "attn.qkv.bias"], G[p + "attn.proj.bias"] = bias_flat[off:off + 3 * D], bias_flat[off + 3 * D:off + 4 * D]
+        G[p + "mlp.fc1.bias"], G[p + "mlp.fc2.bias"] = bias_flat[off + 4 * D:off + 4 * D + Hm], bias_flat[off + 4 * D + Hm:off + 5 * D + Hm]
+        # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod(x_mid))))
+        dm2 = ops.gate_bwd(dxb, m2, g2, rp, dg2, G[p + "mlp.fc2.bias"])
+        G[p + "mlp.fc2.weight"] = self._wgrad(dm2, a)
+        del a
+        # gelu'(u) is a separate pass: in this dgrad's epilogue it made the GEMM the bottleneck (327 us vs 153 + 129 us)
+        da = ops.dgrad(dm2, w2[0])
+        du = ops.gelu_bwd(da, u, G[p + "mlp.fc1.bias"])
+        del da, dm2
+        G[p + "mlp.fc1.weight"] = self._wgrad(du, h2)
+        dh2 = ops.dgrad(du, w1[0])
+        del du
+        ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rp, dxb, dsh2, dsc2)
+        del dh2
+        # x_mid = x_in + g1 * proj(attn(qkv(LNmod(x_in))))
+        dm1 = ops.gate_bwd(dxb, m1, g1, rp, dg1, G[p + "attn.proj.bias"])
+        G[p + "attn.proj.weight"] = self._wgrad(dm1, o)
+        do = ops.dgrad(dm1, wp[0])
+        del dm1
+        dqkv = ops.attention_bwd(qkv, o, do, B, Fr if temporal else Fr + self.images, N, H, temporal)
+        del do
+        ops.colsum(dqkv, G[p + "attn.qkv.bias"])
+        G[p + "attn.qkv.weight"] = self._wgrad(dqkv, h1)
+        dh1 = ops.dgrad(dqkv, wq[0])
+        del dqkv
+        ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rp, dxb, dsh1, dsc1)
+
+    def _wgrad(self, dy, x):
+        g = torch.zeros(dy.shape[1], x.shape[1], dtype=torch.float32, device=dy.device)
+        return self.ops.wgrad(g, dy, x)
+
     def forward(self, x, c, save=True):
         """x (B, F[+I], C, H, W) fp32 -> (B, F[+I], 2C, H, W) fp32.  c: (B, D) fp32 = t_embedder(t) + y_embedder(y)
         (latte.py:332-348) without images, else (B*(F+I), D) per-frame conditioning in row order (`frame_conditioning`).
-        save=False runs the forward without keeping the activations the backward needs."""
+        save=False runs the forward without keeping the activations the backward needs.  With `checkpoint`, each block keeps
+        only its input xs (T x D fp32)."""
         if self.w is None:
             self.prepare()
         m, ops, W = self.m, self.ops, self.w
         B = x.shape[0]
-        D, Fr, N, H = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads
-        T, Tv, rpb, rpb_t = self._geometry(B)
+        D, Fr, N = m.hidden_size, m.num_frames, m.x_embedder.num_patches
+        T, _, rpb, _ = self._geometry(B)
         Fs = Fr + self.images                   # frames a spatial block sees
         dev = x.device
         sc = ops.to_operand(torch.nn.functional.silu(c.float()).contiguous())            # adaLN_modulation[0], final too
         mod = ops.linear(sc, W["ada_w"], W["ada_b"]).float()                               # (B or B(F+I), depth*6D + 2D)
-        mod_t = self._temporal_rows(mod, B)
         S = {"B": B, "c": c, "sc": sc, "mod": mod, "blocks": []}
 
         xp = torch.zeros(T, 64, dtype=torch.float32, device=dev)
@@ -185,33 +300,10 @@ class TrainEngine:
         del xp
         temp = m.temp_embed.detach().float().reshape(Fr, D).contiguous()
         for i in range(m.depth):
-            temporal = bool(i % 2)
-            mv = (mod_t if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-            wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
-            rp = rpb_t if temporal else rpb
-            xi = xs[:Tv] if temporal else xs    # temporal blocks see the video rows only (latte_img.py:373-374, 387-388)
-            h1 = ops.ln_modulate(xi, sh1, sc1, rp)
-            qkv = ops.linear(h1, wq[0], wq[1])
-            o = ops.attention(qkv, B, Fr if temporal else Fs, N, H, temporal)
-            m1 = ops.linear(o, wp[0], wp[1])
-            # two passes: a kernel fusing the residual update with this LayerNorm-modulate measured slower (101 vs 45 + 40 us)
-            xm = ops.gate_residual(xi, m1, g1, rp)
-            h2 = ops.ln_modulate(xm, sh2, sc2, rp)
-            u, a = ops.linear_gelu_both(h2, w1[0], w1[1])
-            m2 = ops.linear(a, w2[0], w2[1])
-            if i == 0 and self.images:
-                # temp_embed goes to the video rows only (latte_img.py:377-378).  All frames of a video share one gate row, so
-                # the video rows take the per-video view, like a temporal block.
-                g2v = mod_t[:, 5 * D:6 * D]
-                xo = self._join_rows(ops.gate_residual(xm[:Tv], m2[:Tv], g2v, rpb_t, row_add=temp, tokens=N),
-                                     ops.gate_residual(xm[Tv:], m2[Tv:], g2[B * Fr:], rp))
-            else:
-                xo = ops.gate_residual(xm, m2, g2, rp, row_add=temp if i == 0 else None, tokens=N)
-                if temporal and self.images:    # image rows pass through the temporal block unchanged
-                    xo = self._join_rows(xo, xs[Tv:])
+            xo, acts = self._block_forward(i, xs, mod, B, temp)
             if save:
-                S["blocks"].append((xi, h1, qkv, o, m1, xm, h2, u, a, m2))
+                S["blocks"].append(xs if self.checkpoint else acts)
+            del acts                            # a checkpointed block's activations are freed before the next block runs
             xs = xo
         base = m.depth * 6 * D
         shf, scf = mod[:, base:base + D], mod[:, base + D:base + 2 * D]
@@ -230,23 +322,16 @@ class TrainEngine:
         m, ops, W, S = self.m, self.ops, self.w, self.saved
         self.saved = None
         B = S["B"]
-        D, Fr, N, H, Hm = m.hidden_size, m.num_frames, m.x_embedder.num_patches, m.num_heads, m.mlp_hidden
-        T, Tv, rpb, rpb_t = self._geometry(B)
+        D, Hm = m.hidden_size, m.mlp_hidden
+        T, _, rpb, _ = self._geometry(B)
         dev = dout.device
         mod = S["mod"]
         G = {}
         dmod = torch.zeros_like(mod)
-        mod_t, dmod_t = self._temporal_rows(mod, B), self._temporal_rows(dmod, B)
         # all bias gradients in one zeroed buffer: per block [qkv 3D | proj D | fc1 Hm | fc2 D], then final (nf), patch (D)
         per_blk = 3 * D + D + Hm + D
         bias_flat = torch.zeros(m.depth * per_blk + self.nf + D, dtype=torch.float32, device=dev)
-
-        def bias_view(i, off, n):
-            return bias_flat[i * per_blk + off: i * per_blk + off + n]
-
-        def wgrad(dy, x):
-            g = torch.zeros(dy.shape[1], x.shape[1], dtype=torch.float32, device=dev)
-            return ops.wgrad(g, dy, x)
+        wgrad = self._wgrad
 
         # ---- final layer (latte.py:197-201) ----
         dtok = self._patchify_out(dout.float())                                         # (T, nf) fp32
@@ -262,46 +347,12 @@ class TrainEngine:
                             dmod[:, base:base + D], dmod[:, base + D:base + 2 * D])
         del dhf, dtp, dtok16
 
-        # ---- blocks, last to first (latte.py:177-181) ----
+        # ---- blocks, last to first (latte.py:177-181); a checkpointed block first reruns its forward from its saved input
         for i in reversed(range(m.depth)):
-            xs, h1, qkv, o, m1, xm, h2, u, a, m2 = S["blocks"].pop()
-            temporal = bool(i % 2)
-            mv = (mod_t if temporal else mod)[:, i * 6 * D:(i + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-            dv = (dmod_t if temporal else dmod)[:, i * 6 * D:(i + 1) * 6 * D]
-            dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
-            rp = rpb_t if temporal else rpb
-            dxb = dx[:Tv] if temporal else dx   # a temporal block passes the image rows' gradient through untouched
-            wq, wp, w1, w2 = (W[f"{i}.{n}"] for n in _BLOCK_LINEARS)
-            p = f"blocks.{i}."
-            G[p + "attn.qkv.bias"], G[p + "attn.proj.bias"] = bias_view(i, 0, 3 * D), bias_view(i, 3 * D, D)
-            G[p + "mlp.fc1.bias"], G[p + "mlp.fc2.bias"] = bias_view(i, 4 * D, Hm), bias_view(i, 4 * D + Hm, D)
-            # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod(x_mid))))
-            dm2 = ops.gate_bwd(dxb, m2, g2, rp, dg2, G[p + "mlp.fc2.bias"])
-            G[p + "mlp.fc2.weight"] = wgrad(dm2, a)
-            del a
-            # gelu'(u) is a separate pass: in this dgrad's epilogue it made the GEMM the bottleneck (327 us vs 153 + 129 us)
-            da = ops.dgrad(dm2, w2[0])
-            du = ops.gelu_bwd(da, u, G[p + "mlp.fc1.bias"])
-            del da, dm2
-            G[p + "mlp.fc1.weight"] = wgrad(du, h2)
-            dh2 = ops.dgrad(du, w1[0])
-            del du
-            ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rp, dxb, dsh2, dsc2)
-            del dh2
-            # x_mid = x_in + g1 * proj(attn(qkv(LNmod(x_in))))
-            dm1 = ops.gate_bwd(dxb, m1, g1, rp, dg1, G[p + "attn.proj.bias"])
-            G[p + "attn.proj.weight"] = wgrad(dm1, o)
-            do = ops.dgrad(dm1, wp[0])
-            del dm1
-            dqkv = ops.attention_bwd(qkv, o, do, B, Fr if temporal else Fr + self.images, N, H, temporal)
-            del do
-            ops.colsum(dqkv, G[p + "attn.qkv.bias"])
-            G[p + "attn.qkv.weight"] = wgrad(dqkv, h1)
-            dh1 = ops.dgrad(dqkv, wq[0])
-            del dqkv
-            ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rp, dxb, dsh1, dsc1)
-            del dh1, xs, h1, qkv, o, m1, xm, h2, u, m2
+            acts = S["blocks"].pop()
+            if self.checkpoint:
+                acts = self._block_forward(i, acts, mod, B, None, rerun=True)[1]
+            self._block_backward(i, acts, dx, mod, dmod, B, G, bias_flat)
 
         # ---- patch embedding (latte.py:330-331; pos_embed / temp_embed are frozen, :246-247) ----
         G["x_embedder.proj.bias"] = ops.colsum(dx, bias_flat[m.depth * per_blk + self.nf:])
@@ -362,8 +413,9 @@ class _LatteTrainFn(torch.autograd.Function):
 
 def train_forward(model, ops, dtype, x, c, images=0):
     """Forward of one training step with the backward attached.  c = t_embedder(t) + y_embedder(y), computed by the caller with
-    torch autograd (a (B, D) graph); with `images` still frames per sample, the per-frame `frame_conditioning` instead."""
-    eng = TrainEngine(model, ops, dtype, images)
+    torch autograd (a (B, D) graph); with `images` still frames per sample, the per-frame `frame_conditioning` instead.
+    Checkpoints each block when `model.gradient_checkpointing` is set."""
+    eng = TrainEngine(model, ops, dtype, images, checkpoint=model.gradient_checkpointing)
     names = trainable_names(model)
     named = dict(model.named_parameters())
     params = [named[n] for n in names]

@@ -35,12 +35,14 @@ class T2VTrainEngine:
     """One training forward + backward of a `LatteT2V` on `ops` with operand type `dtype`.  text (B, L, caption_channels) fp32;
     key_bias None or (B, 128) fp32 additive score bias per caption token ((1 - mask) * -10000, latte_t2v.py:766-771)."""
 
-    def __init__(self, model, ops, dtype, text, key_bias=None):
+    def __init__(self, model, ops, dtype, text, key_bias=None, checkpoint=False):
         self.m = model
         self.ops = ops
         self.dtype = dtype
         self.text = text
         self.key_bias = key_bias
+        #: gradient checkpointing: the forward keeps each block's input only and the backward reruns the block before its backward
+        self.checkpoint = checkpoint
         self.saved = None
         self.w = None
 
@@ -135,6 +137,106 @@ class T2VTrainEngine:
     def _unit(self, n, dev):
         return torch.ones(1, n, dtype=torch.float32, device=dev)
 
+    def _block_forward(self, j, xs, mod, kv, B, temp, rerun=False):
+        """Block j (spatial for even j, temporal for odd j) on its input xs (T x D fp32) -> (its output, the list of
+        activations its backward reads); kv = every layer's caption K/V.  rerun=True is the checkpointed backward's
+        recomputation: it stops before the last residual update, whose output the backward does not read, and returns None
+        in its place."""
+        m, ops, W = self.m, self.ops, self.w
+        D, H = m.inner_dim, m.config.num_attention_heads
+        Fr, N, _ = self._geometry()
+        rpb, L = Fr * N, self.text.shape[1]
+        i, temporal = j // 2, bool(j % 2)
+        mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
+        sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
+        p = f"{'t' if temporal else 's'}{i}."
+        h1 = ops.ln_modulate(xs, sh1, sc1, rpb)
+        qkv = ops.linear(h1, *W[p + "qkv"])
+        o = ops.attention(qkv, B, Fr, N, H, temporal)
+        m1 = ops.linear(o, *W[p + "out"])
+        xm = ops.gate_residual(xs, m1, g1, rpb)
+        cross = None
+        if not temporal:                # x += to_out(attn2(to_q(x), caption K/V))
+            xa = ops.to_operand(xm)
+            q2 = ops.linear(xa, *W[p + "q2"])
+            o2 = ops.cross_attention(q2, kv[:, i * 2 * D:(i + 1) * 2 * D], B, rpb, L, H, self.key_bias)
+            ops.linear_accum(xm, o2, *W[p + "o2"])
+            cross = (xa, q2, o2)
+        h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
+        u, a = ops.linear_gelu_both(h2, *W[p + "fc1"])
+        m2 = ops.linear(a, *W[p + "fc2"])
+        acts = [xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2]
+        if rerun:
+            return None, acts
+        # temp_pos_embed joins after the first spatial block, before the first temporal one (latte_t2v.py:894-895)
+        add = temp if (j == 0 and Fr > 1) else None
+        return ops.gate_residual(xm, m2, g2, rpb, row_add=add, tokens=N), acts
+
+    def _block_backward(self, j, acts, dx, mod, dmod, dkv, kv, unit, B, G):
+        """Backward of block j from the list `_block_forward` returned, which it empties so that each buffer is freed as soon
+        as it is used.  Accumulates into dx (T x D fp32) and dmod, writes the layer's caption dK | dV into dkv and puts the
+        block's weight and bias gradients into G.  Returns dx, which the ungated cross-attention replaces (unit: its gate of
+        ones)."""
+        m, ops, W = self.m, self.ops, self.w
+        D, H = m.inner_dim, m.config.num_attention_heads
+        Fr, N, _ = self._geometry()
+        T, rpb, L = B * Fr * N, Fr * N, self.text.shape[1]
+        xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2 = acts
+        acts.clear()
+        i, temporal = j // 2, bool(j % 2)
+        mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
+        sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
+        dv = dmod[:, j * 6 * D:(j + 1) * 6 * D]
+        dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
+        p = f"{'t' if temporal else 's'}{i}."
+        wgrad, bgrad = self._wgrad, self._bgrad
+        db = {n: bgrad(p + n, dx.device) for n in ("qkv", "out", "fc1", "fc2")}
+        # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod2(x_mid))))
+        dm2 = ops.gate_bwd(dx, m2, g2, rpb, dg2, db["fc2"])
+        G[p + "fc2"] = wgrad(dm2, a)
+        du = ops.gelu_bwd(ops.dgrad(dm2, W[p + "fc2"][0]), u, db["fc1"])
+        del dm2, a
+        G[p + "fc1"] = wgrad(du, h2)
+        dh2 = ops.dgrad(du, W[p + "fc1"][0])
+        del du
+        ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rpb, dx, dsh2, dsc2)
+        del dh2
+        if cross is not None:           # x_mid = x_attn + to_out(attn2(to_q(x_attn)))
+            xa, q2, o2 = cross
+            db["q2"], db["o2"] = bgrad(p + "q2", dx.device), bgrad(p + "o2", dx.device)
+            ops.colsum(dx, db["o2"])
+            dx16 = ops.to_operand(dx)
+            G[p + "o2"] = wgrad(dx16, o2)
+            do2 = ops.dgrad(dx16, W[p + "o2"][0])
+            del dx16
+            dq2 = ops.cross_attention_bwd(q2, kv[:, i * 2 * D:(i + 1) * 2 * D], o2, do2, B, rpb, L, H, self.key_bias, dkv, i * 2 * D)
+            del do2, o2
+            ops.colsum(dq2, db["q2"])
+            G[p + "q2"] = wgrad(dq2, xa)
+            dx = ops.gate_residual(dx, ops.dgrad(dq2, W[p + "q2"][0]), unit, T)
+            del dq2, xa, q2
+        # x_attn = x_in + g1 * out(attn1(qkv(LNmod1(x_in))))
+        dm1 = ops.gate_bwd(dx, m1, g1, rpb, dg1, db["out"])
+        G[p + "out"] = wgrad(dm1, o)
+        do = ops.dgrad(dm1, W[p + "out"][0])
+        del dm1
+        dqkv = ops.attention_bwd(qkv, o, do, B, Fr, N, H, temporal)
+        del do
+        ops.colsum(dqkv, db["qkv"])
+        G[p + "qkv"] = wgrad(dqkv, h1)
+        dh1 = ops.dgrad(dqkv, W[p + "qkv"][0])
+        del dqkv
+        ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rpb, dx, dsh1, dsc1)
+        for n, t in db.items():
+            G[p + n + ".bias"] = t
+        return dx
+
+    def _wgrad(self, dy, x):
+        return self.ops.wgrad(torch.zeros(dy.shape[1], x.shape[1], dtype=torch.float32, device=dy.device), dy, x)
+
+    def _bgrad(self, name, dev):
+        return torch.zeros(self.w[name][1].shape[0], dtype=torch.float32, device=dev)
+
     def forward(self, x, c, save=True):
         """x (B, C, F, H, W) fp32, c = emb (B, D) fp32 -> (B, out_channels, F, H, W) fp32."""
         if self.w is None:
@@ -142,7 +244,7 @@ class T2VTrainEngine:
         m, ops, W = self.m, self.ops, self.w
         cfg = m.config
         B = x.shape[0]
-        D, H, nl = m.inner_dim, cfg.num_attention_heads, cfg.num_layers
+        D, nl = m.inner_dim, cfg.num_layers
         Fr, N, _ = self._geometry()
         T, rpb = B * Fr * N, Fr * N
         L = self.text.shape[1]
@@ -175,30 +277,10 @@ class T2VTrainEngine:
         del xp
         temp = m.temp_pos_embed.detach().float().reshape(-1, D)[:Fr].contiguous()
         for j in range(NB):
-            i, temporal = j // 2, bool(j % 2)
-            mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-            p = f"{'t' if temporal else 's'}{i}."
-            h1 = ops.ln_modulate(xs, sh1, sc1, rpb)
-            qkv = ops.linear(h1, *W[p + "qkv"])
-            o = ops.attention(qkv, B, Fr, N, H, temporal)
-            m1 = ops.linear(o, *W[p + "out"])
-            xm = ops.gate_residual(xs, m1, g1, rpb)
-            cross = None
-            if not temporal:                # x += to_out(attn2(to_q(x), caption K/V))
-                xa = ops.to_operand(xm)
-                q2 = ops.linear(xa, *W[p + "q2"])
-                o2 = ops.cross_attention(q2, kv[:, i * 2 * D:(i + 1) * 2 * D], B, rpb, L, H, self.key_bias)
-                ops.linear_accum(xm, o2, *W[p + "o2"])
-                cross = (xa, q2, o2)
-            h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
-            u, a = ops.linear_gelu_both(h2, *W[p + "fc1"])
-            m2 = ops.linear(a, *W[p + "fc2"])
-            # temp_pos_embed joins after the first spatial block, before the first temporal one (latte_t2v.py:894-895)
-            add = temp if (j == 0 and Fr > 1) else None
-            xo = ops.gate_residual(xm, m2, g2, rpb, row_add=add, tokens=N)
+            xo, acts = self._block_forward(j, xs, mod, kv, B, temp)
             if save:
-                S["blocks"].append((xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2))
+                S["blocks"].append(xs if self.checkpoint else acts)
+            del acts                        # a checkpointed block's activations are freed before the next block runs
             xs = xo
         base = NB * 6 * D
         hf = ops.ln_modulate(xs, mod[:, base:base + D], mod[:, base + D:base + 2 * D], rpb)
@@ -231,23 +313,20 @@ class T2VTrainEngine:
         self.saved = None
         cfg = m.config
         B = S["B"]
-        D, H, nl = m.inner_dim, cfg.num_attention_heads, cfg.num_layers
+        D, nl = m.inner_dim, cfg.num_layers
         NB = 2 * nl
         Fr, N, _ = self._geometry()
         T, rpb = B * Fr * N, Fr * N
-        L = self.text.shape[1]
         Rp = S["kv"].shape[0]
         dev = dout.device
         mod = S["mod"]
         dmod = torch.zeros_like(mod)
         unit = self._unit(D, dev)
         G = {}
-
-        def wgrad(dy, x):
-            return ops.wgrad(torch.zeros(dy.shape[1], x.shape[1], dtype=torch.float32, device=dev), dy, x)
+        wgrad = self._wgrad
 
         def bgrad(name):
-            return torch.zeros(W[name][1].shape[0], dtype=torch.float32, device=dev)
+            return self._bgrad(name, dev)
 
         # ---- output head
         dtok = self._patchify_out(dout.float())
@@ -263,55 +342,12 @@ class T2VTrainEngine:
         del dhf, dtp, dtok
 
         dkv = torch.zeros(Rp, nl * 2 * D, dtype=self.dtype, device=dev)   # every layer's [dK | dV]; padding rows stay zero
+        # blocks, last to first; a checkpointed block first reruns its forward from its saved input
         for j in reversed(range(NB)):
-            xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2 = S["blocks"].pop()
-            i, temporal = j // 2, bool(j % 2)
-            mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
-            sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-            dv = dmod[:, j * 6 * D:(j + 1) * 6 * D]
-            dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
-            p = f"{'t' if temporal else 's'}{i}."
-            db = {n: bgrad(p + n) for n in ("qkv", "out", "fc1", "fc2")}
-            # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod2(x_mid))))
-            dm2 = ops.gate_bwd(dx, m2, g2, rpb, dg2, db["fc2"])
-            G[p + "fc2"] = wgrad(dm2, a)
-            du = ops.gelu_bwd(ops.dgrad(dm2, W[p + "fc2"][0]), u, db["fc1"])
-            del dm2, a
-            G[p + "fc1"] = wgrad(du, h2)
-            dh2 = ops.dgrad(du, W[p + "fc1"][0])
-            del du
-            ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rpb, dx, dsh2, dsc2)
-            del dh2
-            if cross is not None:           # x_mid = x_attn + to_out(attn2(to_q(x_attn)))
-                xa, q2, o2 = cross
-                db["q2"], db["o2"] = bgrad(p + "q2"), bgrad(p + "o2")
-                ops.colsum(dx, db["o2"])
-                dx16 = ops.to_operand(dx)
-                G[p + "o2"] = wgrad(dx16, o2)
-                do2 = ops.dgrad(dx16, W[p + "o2"][0])
-                del dx16
-                dq2 = ops.cross_attention_bwd(q2, S["kv"][:, i * 2 * D:(i + 1) * 2 * D], o2, do2, B, rpb, L, H, self.key_bias,
-                                              dkv, i * 2 * D)
-                del do2, o2
-                ops.colsum(dq2, db["q2"])
-                G[p + "q2"] = wgrad(dq2, xa)
-                dx = ops.gate_residual(dx, ops.dgrad(dq2, W[p + "q2"][0]), unit, T)
-                del dq2, xa, q2
-            # x_attn = x_in + g1 * out(attn1(qkv(LNmod1(x_in))))
-            dm1 = ops.gate_bwd(dx, m1, g1, rpb, dg1, db["out"])
-            G[p + "out"] = wgrad(dm1, o)
-            do = ops.dgrad(dm1, W[p + "out"][0])
-            del dm1
-            dqkv = ops.attention_bwd(qkv, o, do, B, Fr, N, H, temporal)
-            del do
-            ops.colsum(dqkv, db["qkv"])
-            G[p + "qkv"] = wgrad(dqkv, h1)
-            dh1 = ops.dgrad(dqkv, W[p + "qkv"][0])
-            del dqkv
-            ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rpb, dx, dsh1, dsc1)
-            del dh1, xs, h1, qkv, o, m1, xm, h2, u, m2
-            for n, t in db.items():
-                G[p + n + ".bias"] = t
+            acts = S["blocks"].pop()
+            if self.checkpoint:
+                acts = self._block_forward(j, acts, mod, S["kv"], B, None, rerun=True)[1]
+            dx = self._block_backward(j, acts, dx, mod, dmod, dkv, S["kv"], unit, B, G)
 
         # ---- patch embedding (pos_table / temp_pos_embed are frozen buffers)
         G["patch.bias"] = ops.colsum(dx, torch.zeros(D, dtype=torch.float32, device=dev))
@@ -390,8 +426,9 @@ def conditioning(model, t):
 
 
 def train_forward(model, ops, dtype, x, c, text, key_bias=None):
-    """Forward of one training step with the backward attached; c = `conditioning(model, t)`."""
-    eng = T2VTrainEngine(model, ops, dtype, text, key_bias)
+    """Forward of one training step with the backward attached; c = `conditioning(model, t)`.  Checkpoints each block when
+    `model.gradient_checkpointing` is set."""
+    eng = T2VTrainEngine(model, ops, dtype, text, key_bias, checkpoint=model.gradient_checkpointing)
     names = trainable_names(model)
     named = dict(model.named_parameters())
     return _LatteTrainFn.apply(eng, names, x, c, *[named[n] for n in names])
