@@ -13,6 +13,16 @@ the backward collects every layer's dK/dV in one [B*L, layers*2D] buffer (b200_c
 runs one weight gradient and one input gradient over it after the block loop.  Row counts of the caption GEMMs are padded to 64
 with zero rows.
 
+Video + image joint training (`images` = I > 0, latte_t2v.py:730-919 in training mode): each sample is F video frames plus I
+still images, every image with its own caption.  Row order as in `training.TrainEngine`: the B*F*N video rows first, (b, f, n),
+then the B*I*N image rows, (b, i, n).  Caption rows: the B video captions, then the B*I image captions in (b, i) order (the
+stacked K/V, the dK | dV buffer and the key-bias rows follow it).  Spatial blocks and the output head run over every row with
+one modulation row per frame (rows_per_batch = N, each row table_j + ts[b]); each spatial block issues two cross-attention calls
+on row views, the videos (batch B, F*N query rows per caption) and the images (batch B*I, N query rows per caption).  Temporal
+blocks run on the video prefix x[:B*F*N], exactly a batch of B videos, through a strided view with one modulation row per
+video, and carry the image rows through unchanged.  temp_pos_embed is not added (the reference's plain image-joint branch,
+:876-891, has no such term).
+
 `emb` (B, D) stays on torch autograd (a handful of kernels); the engine returns its gradient `dc`, which collects the SiLU path
 into every block's modulation and the output head's direct use of it.  Backend-agnostic: latte_b200.train_ops.NativeOps on the
 GPU, the torch restatement oracle/train_t2v_ops_oracle.T2VTorchOps in the CPU tests.
@@ -33,14 +43,17 @@ def _pad64(n):
 
 class T2VTrainEngine:
     """One training forward + backward of a `LatteT2V` on `ops` with operand type `dtype`.  text (B, L, caption_channels) fp32;
-    key_bias None or (B, 128) fp32 additive score bias per caption token ((1 - mask) * -10000, latte_t2v.py:766-771)."""
+    key_bias None or (B, 128) fp32 additive score bias per caption token ((1 - mask) * -10000, latte_t2v.py:766-771).  With
+    `images` = I > 0 still images per sample, text is (B, 1 + I, L, caption_channels) and key_bias None or (B, 1 + I, 128):
+    caption (b, 0) serves the video frames of sample b, caption (b, 1 + i) its image i (latte_t2v.py:756-762, 791-796)."""
 
-    def __init__(self, model, ops, dtype, text, key_bias=None, checkpoint=False):
+    def __init__(self, model, ops, dtype, text, key_bias=None, checkpoint=False, images=0):
         self.m = model
         self.ops = ops
         self.dtype = dtype
-        self.text = text
-        self.key_bias = key_bias
+        self.images = images
+        self.text = self._caption_rows(text)
+        self.key_bias = self._caption_rows(key_bias)
         #: gradient checkpointing: the forward keeps each block's input only and the backward reruns the block before its backward
         self.checkpoint = checkpoint
         self.saved = None
@@ -134,6 +147,56 @@ class T2VTrainEngine:
         g = c.sample_size // c.patch_size
         return c.video_length, g * g, g
 
+    def _rows(self, B):
+        """(rows of all frames, rows of the video frames, rows_per_batch of spatial blocks / output head, of temporal blocks)."""
+        Fr, N, _ = self._geometry()
+        Tv = B * Fr * N
+        if not self.images:
+            return Tv, Tv, Fr * N, Fr * N
+        return Tv + B * self.images * N, Tv, N, Fr * N
+
+    def _caption_rows(self, t):
+        """(B, 1 + I, ...) per-sample captions -> (B*(1 + I), ...): the B video captions, then the B*I image captions."""
+        if t is None or not self.images:
+            return t
+        return torch.cat((t[:, 0], t[:, 1:].flatten(0, 1))).contiguous()
+
+    def _frame_rows(self, t, B):
+        """Per-sample rows (B, n) -> one row per frame in row order (the video frames, then the images); as is without images."""
+        if not self.images:
+            return t
+        Fr = self._geometry()[0]
+        return torch.cat((t.repeat_interleave(Fr, dim=0), t.repeat_interleave(self.images, dim=0)))
+
+    def _sample_sum(self, t, B):
+        """Adjoint of `_frame_rows`: the rows of each sample's frames summed into one row per sample."""
+        if not self.images:
+            return t
+        Fr = self._geometry()[0]
+        return t[:B * Fr].reshape(B, Fr, -1).sum(1) + t[B * Fr:].reshape(B, self.images, -1).sum(1)
+
+    def _temporal_rows(self, t, B):
+        """The modulation rows (of mod / dmod) a temporal block addresses: per sample without images, else the first frame's row
+        of each video (a strided view)."""
+        Fr = self._geometry()[0]
+        return t[0:B * Fr:Fr] if self.images else t
+
+    def _cross_calls(self, B):
+        """One (query rows, batch, query rows per caption, caption rows) per cross-attention call: the videos, then the images."""
+        Fr, N, _ = self._geometry()
+        L, Tv = self.text.shape[1], B * Fr * N
+        calls = [(slice(0, Tv), B, Fr * N, slice(0, B * L))]
+        if self.images:
+            calls.append((slice(Tv, None), B * self.images, N, slice(B * L, None)))
+        return calls
+
+    def _key_bias(self, nb, rows):
+        """key_bias rows of one cross-attention call (row b*L of the caption buffer <-> key_bias row b)."""
+        if self.key_bias is None:
+            return None
+        L = self.text.shape[1]
+        return self.key_bias[rows.start // L:rows.start // L + nb]
+
     def _unit(self, n, dev):
         return torch.ones(1, n, dtype=torch.float32, device=dev)
 
@@ -145,32 +208,42 @@ class T2VTrainEngine:
         m, ops, W = self.m, self.ops, self.w
         D, H = m.inner_dim, m.config.num_attention_heads
         Fr, N, _ = self._geometry()
-        rpb, L = Fr * N, self.text.shape[1]
+        _, Tv, rpb, rpb_t = self._rows(B)
+        L = self.text.shape[1]
         i, temporal = j // 2, bool(j % 2)
-        mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
+        mv = (self._temporal_rows(mod, B) if temporal else mod)[:, j * 6 * D:(j + 1) * 6 * D]
         sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
         p = f"{'t' if temporal else 's'}{i}."
-        h1 = ops.ln_modulate(xs, sh1, sc1, rpb)
+        rp = rpb_t if temporal else rpb
+        xi = xs[:Tv] if temporal else xs    # temporal blocks see the video rows only (latte_t2v.py:876-891)
+        h1 = ops.ln_modulate(xi, sh1, sc1, rp)
         qkv = ops.linear(h1, *W[p + "qkv"])
-        o = ops.attention(qkv, B, Fr, N, H, temporal)
+        o = ops.attention(qkv, B, Fr if temporal else Fr + self.images, N, H, temporal)
         m1 = ops.linear(o, *W[p + "out"])
-        xm = ops.gate_residual(xs, m1, g1, rpb)
+        xm = ops.gate_residual(xi, m1, g1, rp)
         cross = None
-        if not temporal:                # x += to_out(attn2(to_q(x), caption K/V))
+        if not temporal:                # x += to_out(attn2(to_q(x), caption K/V)), one call per caption group
             xa = ops.to_operand(xm)
             q2 = ops.linear(xa, *W[p + "q2"])
-            o2 = ops.cross_attention(q2, kv[:, i * 2 * D:(i + 1) * 2 * D], B, rpb, L, H, self.key_bias)
+            kvl = kv[:, i * 2 * D:(i + 1) * 2 * D]
+            o2 = [ops.cross_attention(q2[qr], kvl[cr], nb, rows, L, H, self._key_bias(nb, cr))
+                  for qr, nb, rows, cr in self._cross_calls(B)]
+            o2 = o2[0] if len(o2) == 1 else torch.cat(o2)
             ops.linear_accum(xm, o2, *W[p + "o2"])
             cross = (xa, q2, o2)
-        h2 = ops.ln_modulate(xm, sh2, sc2, rpb)
+        h2 = ops.ln_modulate(xm, sh2, sc2, rp)
         u, a = ops.linear_gelu_both(h2, *W[p + "fc1"])
         m2 = ops.linear(a, *W[p + "fc2"])
-        acts = [xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2]
+        acts = [xi, h1, qkv, o, m1, cross, xm, h2, u, a, m2]
         if rerun:
             return None, acts
-        # temp_pos_embed joins after the first spatial block, before the first temporal one (latte_t2v.py:894-895)
-        add = temp if (j == 0 and Fr > 1) else None
-        return ops.gate_residual(xm, m2, g2, rpb, row_add=add, tokens=N), acts
+        # temp_pos_embed joins after the first spatial block, before the first temporal one (latte_t2v.py:894-895); the
+        # image-joint branch adds none (:876-891)
+        add = temp if (j == 0 and Fr > 1 and not self.images) else None
+        xo = ops.gate_residual(xm, m2, g2, rp, row_add=add, tokens=N)
+        if temporal and self.images:        # image rows pass through the temporal block unchanged
+            xo = torch.cat((xo, xs[Tv:]))
+        return xo, acts
 
     def _block_backward(self, j, acts, dx, mod, dmod, dkv, kv, unit, B, G):
         """Backward of block j from the list `_block_forward` returned, which it empties so that each buffer is freed as soon
@@ -180,26 +253,29 @@ class T2VTrainEngine:
         m, ops, W = self.m, self.ops, self.w
         D, H = m.inner_dim, m.config.num_attention_heads
         Fr, N, _ = self._geometry()
-        T, rpb, L = B * Fr * N, Fr * N, self.text.shape[1]
+        T, Tv, rpb, rpb_t = self._rows(B)
+        L = self.text.shape[1]
         xs, h1, qkv, o, m1, cross, xm, h2, u, a, m2 = acts
         acts.clear()
         i, temporal = j // 2, bool(j % 2)
-        mv = mod[:, j * 6 * D:(j + 1) * 6 * D]
+        mv = (self._temporal_rows(mod, B) if temporal else mod)[:, j * 6 * D:(j + 1) * 6 * D]
         sh1, sc1, g1, sh2, sc2, g2 = (mv[:, k * D:(k + 1) * D] for k in range(6))
-        dv = dmod[:, j * 6 * D:(j + 1) * 6 * D]
+        dv = (self._temporal_rows(dmod, B) if temporal else dmod)[:, j * 6 * D:(j + 1) * 6 * D]
         dsh1, dsc1, dg1, dsh2, dsc2, dg2 = (dv[:, k * D:(k + 1) * D] for k in range(6))
         p = f"{'t' if temporal else 's'}{i}."
+        rp = rpb_t if temporal else rpb
+        dxb = dx[:Tv] if temporal else dx   # a temporal block passes the image rows' gradient through untouched
         wgrad, bgrad = self._wgrad, self._bgrad
         db = {n: bgrad(p + n, dx.device) for n in ("qkv", "out", "fc1", "fc2")}
         # x_out = x_mid + g2 * fc2(gelu(fc1(LNmod2(x_mid))))
-        dm2 = ops.gate_bwd(dx, m2, g2, rpb, dg2, db["fc2"])
+        dm2 = ops.gate_bwd(dxb, m2, g2, rp, dg2, db["fc2"])
         G[p + "fc2"] = wgrad(dm2, a)
         du = ops.gelu_bwd(ops.dgrad(dm2, W[p + "fc2"][0]), u, db["fc1"])
         del dm2, a
         G[p + "fc1"] = wgrad(du, h2)
         dh2 = ops.dgrad(du, W[p + "fc1"][0])
         del du
-        ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rpb, dx, dsh2, dsc2)
+        ops.ln_modulate_bwd(dh2, xm, sh2, sc2, rp, dxb, dsh2, dsc2)
         del dh2
         if cross is not None:           # x_mid = x_attn + to_out(attn2(to_q(x_attn)))
             xa, q2, o2 = cross
@@ -209,24 +285,27 @@ class T2VTrainEngine:
             G[p + "o2"] = wgrad(dx16, o2)
             do2 = ops.dgrad(dx16, W[p + "o2"][0])
             del dx16
-            dq2 = ops.cross_attention_bwd(q2, kv[:, i * 2 * D:(i + 1) * 2 * D], o2, do2, B, rpb, L, H, self.key_bias, dkv, i * 2 * D)
+            kvl = kv[:, i * 2 * D:(i + 1) * 2 * D]
+            dq2 = [ops.cross_attention_bwd(q2[qr], kvl[cr], o2[qr], do2[qr], nb, rows, L, H, self._key_bias(nb, cr), dkv[cr],
+                                           i * 2 * D) for qr, nb, rows, cr in self._cross_calls(B)]
+            dq2 = dq2[0] if len(dq2) == 1 else torch.cat(dq2)
             del do2, o2
             ops.colsum(dq2, db["q2"])
             G[p + "q2"] = wgrad(dq2, xa)
-            dx = ops.gate_residual(dx, ops.dgrad(dq2, W[p + "q2"][0]), unit, T)
+            dx = dxb = ops.gate_residual(dx, ops.dgrad(dq2, W[p + "q2"][0]), unit, T)
             del dq2, xa, q2
         # x_attn = x_in + g1 * out(attn1(qkv(LNmod1(x_in))))
-        dm1 = ops.gate_bwd(dx, m1, g1, rpb, dg1, db["out"])
+        dm1 = ops.gate_bwd(dxb, m1, g1, rp, dg1, db["out"])
         G[p + "out"] = wgrad(dm1, o)
         do = ops.dgrad(dm1, W[p + "out"][0])
         del dm1
-        dqkv = ops.attention_bwd(qkv, o, do, B, Fr, N, H, temporal)
+        dqkv = ops.attention_bwd(qkv, o, do, B, Fr if temporal else Fr + self.images, N, H, temporal)
         del do
         ops.colsum(dqkv, db["qkv"])
         G[p + "qkv"] = wgrad(dqkv, h1)
         dh1 = ops.dgrad(dqkv, W[p + "qkv"][0])
         del dqkv
-        ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rpb, dx, dsh1, dsc1)
+        ops.ln_modulate_bwd(dh1, xs, sh1, sc1, rp, dxb, dsh1, dsc1)
         for n, t in db.items():
             G[p + n + ".bias"] = t
         return dx
@@ -238,7 +317,7 @@ class T2VTrainEngine:
         return torch.zeros(self.w[name][1].shape[0], dtype=torch.float32, device=dev)
 
     def forward(self, x, c, save=True):
-        """x (B, C, F, H, W) fp32, c = emb (B, D) fp32 -> (B, out_channels, F, H, W) fp32."""
+        """x (B, C, F[+I], H, W) fp32, c = emb (B, D) fp32 -> (B, out_channels, F[+I], H, W) fp32."""
         if self.w is None:
             self.prepare()
         m, ops, W = self.m, self.ops, self.w
@@ -246,15 +325,18 @@ class T2VTrainEngine:
         B = x.shape[0]
         D, nl = m.inner_dim, cfg.num_layers
         Fr, N, _ = self._geometry()
-        T, rpb = B * Fr * N, Fr * N
+        T, _, rpb, _ = self._rows(B)
         L = self.text.shape[1]
-        R, Rp = B * L, _pad64(B * L)
+        R = self.text.shape[0] * L
+        Rp = _pad64(R)
         dev = x.device
         # ---- conditioning: ts = adaln_single.linear(silu(emb)); block j's six rows = table_j + ts; output head = table_f + emb
+        # (one row per sample, or per frame with images: the conditioning stays per sample, latte_t2v.py:801, :919)
         sc = ops.to_operand(F.silu(c.float()).contiguous())
         ts = ops.linear(sc, *W["ada"]).float()                                             # (B, 6D)
         NB = 2 * nl
-        mod = torch.cat((W["tables"] + ts.repeat(1, NB), W["final_table"] + c.float().repeat(1, 2)), dim=1).contiguous()
+        mod = torch.cat((W["tables"] + self._frame_rows(ts, B).repeat(1, NB),
+                         W["final_table"] + self._frame_rows(c.float(), B).repeat(1, 2)), dim=1).contiguous()
         S = {"B": B, "c": c, "sc": sc, "mod": mod, "blocks": []}
         # ---- caption projection (B*L rows, padded to 64) and every layer's K/V in one GEMM
         tp = torch.zeros(Rp, self.text.shape[2], dtype=torch.float32, device=dev)
@@ -268,9 +350,14 @@ class T2VTrainEngine:
             S.update(text16=text16, cu=cu, ca=ca, txt=txt, kv=kv)
         # ---- patch embedding + the frozen sin-cos table
         xp = torch.zeros(T, 64, dtype=torch.float32, device=dev)
-        xp[:, : self.kp] = _patch_rows(x.float().permute(0, 2, 1, 3, 4), cfg.patch_size)
+        xf = x.float().permute(0, 2, 1, 3, 4)
+        if self.images:
+            xp[:, : self.kp] = torch.cat((_patch_rows(xf[:, :Fr], cfg.patch_size), _patch_rows(xf[:, Fr:], cfg.patch_size)))
+        else:
+            xp[:, : self.kp] = _patch_rows(xf, cfg.patch_size)
+        del xf
         xp = ops.to_operand(xp)
-        xs = m.pos_table.detach().float().reshape(1, N, D).expand(B * Fr, N, D).reshape(T, D).contiguous()
+        xs = m.pos_table.detach().float().reshape(1, N, D).expand(B * (Fr + self.images), N, D).reshape(T, D).contiguous()
         ops.linear_accum(xs, xp, *W["patch"])
         if save:
             S["xp"] = xp
@@ -291,32 +378,42 @@ class T2VTrainEngine:
         return self._unpatchify(tok, B)
 
     def _unpatchify(self, tok, B):
-        """rows (b, f, h, w) x (p, q, c) -> (B, c, F, h*p, w*q) (latte_t2v.py:929-936)."""
+        """rows (b, f, h, w) x (p, q, c) -> (B, c, F, h*p, w*q) (latte_t2v.py:929-936); image rows follow as frames F.."""
         cfg = self.m.config
-        Fr, _, g = self._geometry()
+        Fr, N, g = self._geometry()
         p, c = cfg.patch_size, cfg.out_channels
-        t = tok.view(B * Fr, g, g, p, p, c).permute(0, 5, 1, 3, 2, 4).reshape(B, Fr, c, g * p, g * p)
-        return t.permute(0, 2, 1, 3, 4)
+
+        def unp(rows, frames):
+            t = rows.view(B * frames, g, g, p, p, c).permute(0, 5, 1, 3, 2, 4).reshape(B, frames, c, g * p, g * p)
+            return t.permute(0, 2, 1, 3, 4)
+        if self.images:
+            Tv = B * Fr * N
+            return torch.cat((unp(tok[:Tv], Fr), unp(tok[Tv:], self.images)), dim=2)
+        return unp(tok, Fr)
 
     def _patchify_out(self, dout):
         cfg = self.m.config
         Fr, _, g = self._geometry()
         p, c = cfg.patch_size, cfg.out_channels
-        B = dout.shape[0]
-        t = dout.permute(0, 2, 1, 3, 4).reshape(B * Fr, c, g, p, g, p).permute(0, 2, 4, 3, 5, 1)
-        return t.reshape(B * Fr * g * g, p * p * c).contiguous()
+
+        def pat(d):
+            B, frames = d.shape[0], d.shape[2]
+            t = d.permute(0, 2, 1, 3, 4).reshape(B * frames, c, g, p, g, p).permute(0, 2, 4, 3, 5, 1)
+            return t.reshape(B * frames * g * g, p * p * c)
+        if self.images:
+            return torch.cat((pat(dout[:, :, :Fr]), pat(dout[:, :, Fr:])))
+        return pat(dout).contiguous()
 
     # ---------------------------------------------------------------------------------------------------------------
     def backward(self, dout):
-        """dout (B, c, F, H, W) -> ({parameter name: fp32 gradient}, dc (B, D) fp32).  Frees the saved activations."""
+        """dout (B, c, F[+I], H, W) -> ({parameter name: fp32 gradient}, dc (B, D) fp32).  Frees the saved activations."""
         m, ops, W, S = self.m, self.ops, self.w, self.saved
         self.saved = None
         cfg = m.config
         B = S["B"]
         D, nl = m.inner_dim, cfg.num_layers
         NB = 2 * nl
-        Fr, N, _ = self._geometry()
-        T, rpb = B * Fr * N, Fr * N
+        T, _, rpb, _ = self._rows(B)
         Rp = S["kv"].shape[0]
         dev = dout.device
         mod = S["mod"]
@@ -368,13 +465,13 @@ class T2VTrainEngine:
 
         # ---- conditioning: block tables, ts = linear(silu(emb)), output head's direct use of emb
         dtab = dmod[:, :base].sum(0)
-        dts = dmod[:, :base].reshape(B, NB, 6 * D).sum(1).contiguous()
+        dts = self._sample_sum(dmod[:, :base], B).reshape(B, NB, 6 * D).sum(1).contiguous()
         G["ada"] = ops.ada_outer(dts, S["sc"])
         G["ada.bias"] = dts.sum(0)
         dsc = ops.ada_dsc(dts, W["ada"][0])
         c = S["c"].float()
         sg = torch.sigmoid(c)
-        dfin = dmod[:, base:]
+        dfin = self._sample_sum(dmod[:, base:], B)
         dc = dsc * (sg * (1 + c * (1 - sg))) + dfin[:, :D] + dfin[:, D:]
         return self._named(G, dtab, dfin.sum(0)), dc
 
@@ -425,10 +522,11 @@ def conditioning(model, t):
     return te.linear_2(F.silu(te.linear_1(e.to(te.linear_1.weight.dtype)))).float()
 
 
-def train_forward(model, ops, dtype, x, c, text, key_bias=None):
-    """Forward of one training step with the backward attached; c = `conditioning(model, t)`.  Checkpoints each block when
-    `model.gradient_checkpointing` is set."""
-    eng = T2VTrainEngine(model, ops, dtype, text, key_bias, checkpoint=model.gradient_checkpointing)
+def train_forward(model, ops, dtype, x, c, text, key_bias=None, images=0):
+    """Forward of one training step with the backward attached; c = `conditioning(model, t)`.  With `images` still images per
+    sample, x is (B, C, F + images, H, W) and text / key_bias carry 1 + images captions per sample (see T2VTrainEngine).
+    Checkpoints each block when `model.gradient_checkpointing` is set."""
+    eng = T2VTrainEngine(model, ops, dtype, text, key_bias, checkpoint=model.gradient_checkpointing, images=images)
     names = trainable_names(model)
     named = dict(model.named_parameters())
     return _LatteTrainFn.apply(eng, names, x, c, *[named[n] for n in names])
