@@ -1118,6 +1118,9 @@ __global__ void __launch_bounds__(128) attn_bwd_temporal_mma_kernel(const uint16
     }
   };
   const float scale = scale_log2 * 0.6931471805599453f;
+  // fp16 keeps the softmax scale out of the 16-bit dS operands and applies it to the fp32 dQ / dK (see kernel A above)
+  constexpr bool DEFER = !BF16;
+  const float ds_scale = DEFER ? 1.0f : scale;
   const int c_lo = (lane & 3) * 2;                 // this thread's columns: c_lo, c_lo+1 (n-tile 0), +8 (n-tile 1)
   // ---- orientation 1: rows = queries
   float s[2][4] = {}, dp[2][4] = {};
@@ -1169,7 +1172,7 @@ __global__ void __launch_bounds__(128) attn_bwd_temporal_mma_kernel(const uint16
 #pragma unroll
     for (int t = 0; t < 2; ++t)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) t0[t][e] = s[t][e] * (dp[t][e] - dl[e >> 1]) * scale;
+      for (int e = 0; e < 4; ++e) t0[t][e] = s[t][e] * (dp[t][e] - dl[e >> 1]) * ds_scale;
     ds_a[0] = pack2<BF16>(t0[0][0], t0[0][1]); ds_a[1] = pack2<BF16>(t0[0][2], t0[0][3]);
     ds_a[2] = pack2<BF16>(t0[1][0], t0[1][1]); ds_a[3] = pack2<BF16>(t0[1][2], t0[1][3]);
   }
@@ -1205,7 +1208,7 @@ __global__ void __launch_bounds__(128) attn_bwd_temporal_mma_kernel(const uint16
         const int qi = t * 8 + c_lo + (e & 1);
         const float pr = exp2f(st[t][e] * scale_log2 - sL[qi]);
         pv[t][e] = pr;
-        dv_[t][e] = pr * (dpt[t][e] - sL[16 + qi]) * scale;
+        dv_[t][e] = pr * (dpt[t][e] - sL[16 + qi]) * ds_scale;
       }
     pt_a[0] = pack2<BF16>(pv[0][0], pv[0][1]); pt_a[1] = pack2<BF16>(pv[0][2], pv[0][3]);
     pt_a[2] = pack2<BF16>(pv[1][0], pv[1][1]); pt_a[3] = pack2<BF16>(pv[1][2], pv[1][3]);
@@ -1215,6 +1218,15 @@ __global__ void __launch_bounds__(128) attn_bwd_temporal_mma_kernel(const uint16
   float dk[G::NT][4] = {}, dv[G::NT][4] = {};
   mm_out(dv, pt_a, sG);
   mm_out(dk, dst_a, sQ);
+  if constexpr (DEFER) {
+#pragma unroll
+    for (int nn = 0; nn < G::NT; ++nn)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        dq[nn][e] *= scale;
+        dk[nn][e] *= scale;
+      }
+  }
   __syncwarp();
   // ---- stage the three results in the q / k / v tiles, then 16-byte stores
   auto stage = [&](uint16_t* tile, const float (&acc)[G::NT][4]) {
