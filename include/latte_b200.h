@@ -380,7 +380,8 @@ B200_API int b200_ln_modulate(const float* x, const float* shift, const float* s
  * The reference differentiates Latte.forward with torch autograd; the replacement keeps the same forward kernels, stores the
  * activations, and evaluates the analytic backward with b200_linear (every dgrad: A = dY, W = W^T; every wgrad: A = dY^T,
  * W = X^T, B200_EPI_GATE_RESIDUAL with a unit gate accumulating into the fp32 gradient) plus the passes below.  Host side:
- * latte_b200/training.py (TrainEngine).  All [rows, dim] matrices are row-major; "16" = fp16/bf16 per `dtype`.           */
+ * latte_b200/training.py (the engine base and TrainEngine; T2VTrainEngine in training_t2v.py adds the cross-attention
+ * entries).  All [rows, dim] matrices are row-major; "16" = fp16/bf16 per `dtype`.                                        */
 /* dW[n_out, n_in] (fp32, in place) += col_scale[n_in] * (dY16[rows, n_out]^T . X16[rows, n_in]) -- the weight gradient of
  * Y = X W^T, reading both activations as they lie in memory (the GEMM's MN-major operand mode: no transposed copies),
  * accumulated in fp32 through the residual epilogue (sk_flags as in b200_linear).  col_scale: n_in floats, 1.0 for a plain

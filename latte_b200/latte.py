@@ -335,7 +335,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         `loss.backward()`, optimizer, `clip_grad_norm_` and DistributedDataParallel work unchanged.  Operands are bf16 under
         `torch.autocast(bfloat16)` / fp32 parameters (the reference's mixed-precision recipe) or the parameter dtype if that is
         16-bit; accumulation, the residual stream, LayerNorm statistics and every gradient buffer are fp32."""
-        from . import training, train_ops
+        from . import training
         if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[2] != self.in_channels \
                 or x.shape[3] != self.input_size or x.shape[4] != self.input_size:
             raise ValueError(f"x must be (B, {self.num_frames}, {self.in_channels}, {self.input_size}, {self.input_size}), got {tuple(x.shape)}")
@@ -343,12 +343,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         if self.pos_embed.device != dev:
             raise RuntimeError(f"model is on {self.pos_embed.device}, input on {dev}")
         _lib.load()
-        pd = self.blocks[0].attn.qkv.weight.dtype
-        od = pd if pd in (torch.float16, torch.bfloat16) else self.train_dtype
-        if torch.is_autocast_enabled("cuda"):
-            od = torch.get_autocast_dtype("cuda")
-            if od not in (torch.float16, torch.bfloat16):
-                raise TypeError(f"latte_b200: autocast dtype {od} is not a tensor-core operand type")
+        od, ops = training.native_backend(self, self.blocks[0].attn.qkv.weight.dtype)
         B = x.shape[0]
         tt = t.to(device=dev, dtype=torch.int64)
         yy = None
@@ -359,11 +354,6 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             if self.y_embedder.dropout_prob > 0:                        # token_drop, latte.py:137-146
                 drop = torch.rand(B, device=dev) < self.y_embedder.dropout_prob
                 yy = torch.where(drop, torch.full_like(yy, self.y_embedder.num_classes), yy)
-        ops = self._train_backend.get(od) if self._train_backend else None
-        if ops is None:                         # one backend object per operand type: it caches the multi-cast pointer table
-            if self._train_backend is None:
-                self._train_backend = {}
-            ops = self._train_backend[od] = train_ops.NativeOps(od)
         with torch.autocast("cuda", enabled=False):
             c = training.conditioning(self, tt, yy)
             return training.train_forward(self, ops, od, x.float(), c)

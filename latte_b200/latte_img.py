@@ -73,7 +73,7 @@ class LatteIMG(Latte):
             raise RuntimeError(f"model is on {self.pos_embed.device}, input on {dev}")
         from . import training
         _lib.load()
-        od, ops = self._train_ops()
+        od, ops = training.native_backend(self, self.blocks[0].attn.qkv.weight.dtype)
         with torch.autocast("cuda", enabled=False):
             if train_step:
                 c = training.frame_conditioning(self, tt, yy, yi, I)
@@ -103,23 +103,6 @@ class LatteIMG(Latte):
         if yi.dtype.is_floating_point or yi.dtype == torch.bool:
             raise ValueError(f"y_image holds class labels (an integer type), got {yi.dtype}")
         return yi.to(device=dev, dtype=torch.int64)
-
-    def _train_ops(self):
-        """Operand type and native backend of the engine: the parameter dtype if 16-bit, else bf16 (`train_dtype`) or the
-        autocast dtype, exactly as `Latte`'s training step chooses them."""
-        from . import train_ops
-        pd = self.blocks[0].attn.qkv.weight.dtype
-        od = pd if pd in (torch.float16, torch.bfloat16) else self.train_dtype
-        if torch.is_autocast_enabled("cuda"):
-            od = torch.get_autocast_dtype("cuda")
-            if od not in (torch.float16, torch.bfloat16):
-                raise TypeError(f"latte_b200: autocast dtype {od} is not a tensor-core operand type")
-        if self._train_backend is None:
-            self._train_backend = {}
-        ops = self._train_backend.get(od)
-        if ops is None:
-            ops = self._train_backend[od] = train_ops.NativeOps(od)
-        return od, ops
 
 
 def _mk(depth, hidden, patch, heads):

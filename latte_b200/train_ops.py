@@ -1,6 +1,7 @@
-"""Native backend of latte_b200.training.TrainEngine: every op is one C-ABI call into liblatte_b200.so (csrc/train.cu for the
-backward passes, the wgmma GEMM / attention / LayerNorm kernels of the sampling path for the rest).  CUDA only — a CPU tensor
-raises; the torch restatement of the same ops lives in oracle/train_ops_oracle.py and is test infrastructure."""
+"""Native backend of the training engines (latte_b200.training.TrainEngine, training_t2v.T2VTrainEngine): every op is one
+C-ABI call into liblatte_b200.so (csrc/train.cu for the backward passes and the cross-attention, the wgmma GEMM / attention /
+LayerNorm kernels of the sampling path for the rest).  CUDA only — a CPU tensor raises; the torch restatements of the same
+ops live in oracle/train_ops_oracle.py and oracle/train_t2v_ops_oracle.py and are test infrastructure."""
 from __future__ import annotations
 
 import torch

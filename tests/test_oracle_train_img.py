@@ -8,6 +8,7 @@ first, image rows after), the per-frame conditioning and the temporal blocks' vi
 the factory, the parameters that receive gradients and the input checks."""
 import inspect
 import os
+import weakref
 from types import SimpleNamespace
 
 import numpy as np
@@ -103,6 +104,30 @@ def test_engine_forward_only_equals_training_forward(golden_dir):
     assert torch.equal(a, b)
     want = latte_img_forward(sd, cfg, x0, t, y, yi, I)
     assert (a - want).abs().max().item() <= 1e-4 * want.abs().max().item()
+
+
+def test_engine_forward_only_frees_each_block_before_the_next(golden_dir):
+    """The no-grad forward keeps no activations: when a block (or the output head) starts, the activations of the blocks
+    before it are already freed -- the peak stays at one block's, not the whole model's training activations."""
+    g, cfg, sd, m = _setup(golden_dir, 2)
+    x0, _, t, y, yi = _inputs(g)
+    ops = TorchOps(torch.float32)
+    made, alive = [], []
+    gelu_both, ln_modulate = ops.linear_gelu_both, ops.ln_modulate
+
+    def tracked_gelu_both(*a):
+        u, act = gelu_both(*a)
+        made.extend((weakref.ref(u), weakref.ref(act)))
+        return u, act
+
+    def tracked_ln_modulate(*a):
+        alive.append(sum(r() is not None for r in made))
+        return ln_modulate(*a)
+    ops.linear_gelu_both, ops.ln_modulate = tracked_gelu_both, tracked_ln_modulate
+    with torch.no_grad():
+        training.image_forward(m, ops, torch.float32, x0, training.frame_conditioning(m, t, y, yi, I), I)
+    assert len(made) == 2 * m.depth and len(alive) == 2 * m.depth + 1
+    assert alive == [0] * len(alive)
 
 
 def test_frame_conditioning_matches_reference_per_frame_rows():
