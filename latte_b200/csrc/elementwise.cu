@@ -499,7 +499,8 @@ __global__ void cfg_combine_kernel(float* __restrict__ out, int half_batch, long
     if (c < guided_ch) {
       const float cond = out[i];
       const float uncond = out[i + total];
-      const float e = uncond + scale * (cond - uncond);
+      // the product is rounded before the add, as the reference's fp32 tensor expression rounds it (no fma contraction)
+      const float e = __fadd_rn(uncond, __fmul_rn(scale, __fsub_rn(cond, uncond)));
       out[i] = e;
       out[i + total] = e;
     }

@@ -33,15 +33,11 @@ import math
 import pytest
 import torch
 
+from fp64_bounds import A, B, DTS, LOG2E, SUB, TANH_U, U16, U32, Checker, report_worst  # noqa: E402
+from fp64_bounds import edge_rows as _edge_rows, sqfloor as _sqfloor, to_rows as _to_rows, to_seq as _to_seq  # noqa: E402
+
 pytestmark = pytest.mark.gpu
 
-DTS = [torch.float16, torch.bfloat16]
-U16 = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}
-U32 = 2.0 ** -24
-SUB = {torch.float16: 2.0 ** -24, torch.bfloat16: 0.0}     # subnormal spacing of the 16-bit type (bf16: none that matters)
-TANH_U = 2.0 ** -11                                          # tanh.approx.f32 relative error
-LOG2E = 1.4426950408889634
-A, B, F = 2.0, 4.0, 3.0
 SCALES = {"unit": 1.0, "train": 2.0 ** -20, "fp16-loss-scaled": 2.0 ** -20 * 2.0 ** 16}
 GELU_K0, GELU_K1 = 0.7978845608028654, 0.044715
 
@@ -56,10 +52,7 @@ def dev():
 @pytest.fixture(scope="module", autouse=True)
 def _report_worst():
     yield
-    if _WORST:
-        print("\nworst err / bound per op and dtype:")
-        for (op, dt), (r, where) in sorted(_WORST.items()):
-            print(f"  {op:<34} {dt:<9} {r:8.3g}   {where}")
+    report_worst(_WORST)
 
 
 def _nat(dt):
@@ -67,36 +60,8 @@ def _nat(dt):
     return NativeOps(dt)
 
 
-def _dtn(dt):
-    return str(dt).replace("torch.", "")
-
-
-class _Checker:
-    """Compares every output of one test, keeps the module-wide worst err / bound per op and dtype, and fails at the end
-    listing every output above 1 with its location."""
-
-    def __init__(self, dt):
-        self.dt, self.bad = dt, []
-
-    def add(self, op, what, got, ref, bound, where):
-        got = got.double()
-        err = (got - ref).abs()
-        ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300),
-                            torch.where(err > 0, torch.full_like(err, math.inf), torch.zeros_like(err)))
-        ratio = torch.where(torch.isfinite(got), ratio, torch.full_like(ratio, math.inf))
-        i = int(torch.argmax(ratio).item())
-        r = float(ratio.reshape(-1)[i].item())
-        idx = [int(v) for v in torch.unravel_index(torch.tensor(i), ratio.shape)]
-        loc = (f"{what} at {where(idx)}: got {got.reshape(-1)[i].item():.6g}, ref {ref.reshape(-1)[i].item():.6g}, "
-               f"bound {bound.reshape(-1)[i].item():.3g}")
-        key = (op, _dtn(self.dt))
-        if key not in _WORST or r > _WORST[key][0]:
-            _WORST[key] = (r, loc)
-        if r > 1.0:
-            self.bad.append(f"{op} {loc}: err/bound {r:.3g}")
-
-    def done(self):
-        assert not self.bad, "\n".join(self.bad[:12])
+def _Checker(dt):
+    return Checker(dt, _WORST)
 
 
 def _rc(idx):
@@ -109,14 +74,6 @@ def _sc(idx):
 
 def _col(idx):
     return f"column {idx[0]}"
-
-
-def _sqfloor(x, y, s, lhs_t=False):
-    """F * sqrt(sum_k (min(s, |x|) * |y|)^2) as a matrix product: x [.., m, k] (or [.., k, m] with lhs_t), y [.., k, n]."""
-    xm = x.abs().clamp_max(s) ** 2
-    if lhs_t:
-        xm = xm.transpose(-1, -2)
-    return F * (xm @ (y * y)).sqrt()
 
 
 # ------------------------------------------------------------------------------------------------ elementwise backward ops
@@ -358,40 +315,6 @@ def _softmax_bwd_terms(q, k, v, do, bias, dt):
             terms["dk"] += sc * _sqfloor(mdS, q, SUB[dt], lhs_t=True) + SUB[dt]
             terms["dv"] += _sqfloor(P, do, SUB[dt], lhs_t=True) + SUB[dt]
     return out, terms
-
-
-def _to_seq(t, Bb, Fr, N, parts, H, hd, temporal):
-    """[B*F*N, parts*H*hd] rows (b, f, n) -> [sequences, parts, H, S, hd]: spatial sequences (b, f) over n, temporal (b, n)
-    over f."""
-    x = t.reshape(Bb, Fr, N, parts, H, hd)
-    if temporal:
-        return x.permute(0, 2, 3, 4, 1, 5).reshape(Bb * N, parts, H, Fr, hd)
-    return x.permute(0, 1, 3, 4, 2, 5).reshape(Bb * Fr, parts, H, N, hd)
-
-
-def _to_rows(x, Bb, Fr, N, H, hd, temporal):
-    parts = x.shape[1]
-    if temporal:
-        return x.reshape(Bb, N, parts, H, Fr, hd).permute(0, 4, 1, 2, 3, 5).reshape(Bb * Fr * N, parts * H * hd)
-    return x.reshape(Bb, Fr, parts, H, N, hd).permute(0, 1, 4, 2, 3, 5).reshape(Bb * Fr * N, parts * H * hd)
-
-
-def _edge_rows(x):
-    """x [sequences, 3, H, S, hd] (q | k | v): query 0 peaks at the LAST key (logit 30), query 1 is constant (q = 0), query 2
-    has logits +30 at the middle key and -30 at key 0, query 3 shares its maximum between keys 1 and S - 2."""
-    S, hd = x.shape[3], x.shape[4]
-    k = x[:, 1]
-
-    def toward(j, logit):
-        kj = k[:, :, j]
-        return kj * (logit * math.sqrt(hd) / (kj * kj).sum(-1, keepdim=True))
-    x[:, 0, :, 0] = toward(S - 1, 30.0)
-    if S > 1:
-        x[:, 0, :, 1] = 0
-    if S > 2:
-        x[:, 0, :, 2] = toward(S // 2, 30.0) + toward(0, -30.0)
-    if S > 3:
-        x[:, 0, :, 3] = toward(1, 12.0) + toward(S - 2, 12.0)
 
 
 def _attention_case(dev, dt, Bb, Fr, N, H, hd, temporal):
