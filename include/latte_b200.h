@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 4
+#define B200_ABI_VERSION 5
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
 #else
@@ -73,11 +73,11 @@ typedef struct B200LatteWeights {
   const float* y_table;    /* y_embedder.embedding_table.weight [num_embed, D] or NULL    */
   const void* ada_w16;     /* blocks.*.adaLN_modulation.1.weight then final_layer's: [depth*6D + 2D, D] 16-bit */
   const float* ada_b;      /* matching biases             [depth*6D + 2D]                 */
-  const void* qkv_w16;     /* blocks.*.attn.qkv.weight    [depth][3D, D] 16-bit           */
+  const void* qkv_w16;     /* blocks.*.attn.qkv.weight    [depth][3D, D] 16-bit (NULL allowed when qkv_w8 is set) */
   const float* qkv_b;      /*                             [depth][3D]                     */
   const void* proj_w16;    /* blocks.*.attn.proj.weight   [depth][D, D] 16-bit            */
   const float* proj_b;     /*                             [depth][D]                      */
-  const void* fc1_w16;     /* blocks.*.mlp.fc1.weight     [depth][4D, D] 16-bit           */
+  const void* fc1_w16;     /* blocks.*.mlp.fc1.weight     [depth][4D, D] 16-bit (NULL allowed when fc1_w8 is set) */
   const float* fc1_b;      /*                             [depth][4D]                     */
   const void* fc2_w16;     /* blocks.*.mlp.fc2.weight     [depth][D, 4D] 16-bit           */
   const float* fc2_b;      /*                             [depth][D]                      */
@@ -85,6 +85,14 @@ typedef struct B200LatteWeights {
   const float* final_b;    /* final_layer.linear.bias     [p*p*out_channels]              */
   const void* final_w16;   /* 16-bit copy of final_w: the head then runs LN+modulate -> wgmma GEMM (N = p*p*out_channels,
                               fp32 result) -> unpatchify; NULL keeps the fp32 CUDA-core head                 */
+  /* FP8 sampling path (opt-in; NULL = the 16-bit GEMM).  e4m3 copies of qkv_w16 / fc1_w16's weights with one fp32 scale per
+   * output channel, as b200_quantize_rows_e4m3 makes them.  When set, that block GEMM's LayerNorm + modulate writes e4m3
+   * with one scale per token and the GEMM multiplies e4m3 on the tensor cores; every other operand stays 16-bit.
+   * The 16-bit copy of a weight that has an e4m3 copy is not read.                                                      */
+  const void* qkv_w8;      /* blocks.*.attn.qkv.weight    [depth][3D, D] e4m3             */
+  const float* qkv_ws;     /*                             [depth][3D] scales              */
+  const void* fc1_w8;      /* blocks.*.mlp.fc1.weight     [depth][4D, D] e4m3             */
+  const float* fc1_ws;     /*                             [depth][4D] scales              */
 } B200LatteWeights;
 
 /* ---- LatteT2V (reference models/latte_t2v.py:444-944, HF maxin-cn/Latte-1 config: ada_norm_single, gelu-approximate,
@@ -375,6 +383,21 @@ B200_API int b200_attention(const void* qkv, void* out, int batch, int frames, i
  * — replaces norm1/norm2 + modulate (latte.py:28-29, 166-168, 179-180). x fp32 [rows, dim].          */
 B200_API int b200_ln_modulate(const float* x, const float* shift, const float* scale, int64_t mod_batch_stride,
                      int rows_per_batch, void* out16, int rows, int dim, int dtype, void* stream);
+
+/* ---- FP8 (e4m3) sampling path.  One formula quantizes both operands, row by row:
+ *   s = amax(|row|) / 448 (1 for an all-zero row),  q = e4m3_rn_satfinite(row / s)  (fp32, correctly rounded division)
+ * b200_quantize_rows_e4m3: w fp32 [rows, cols] -> q8 [rows, cols] e4m3 bytes, scales [rows] fp32 (a weight W[N, K]: one
+ *   scale per output channel).  cols % 16 == 0; w, q8 16-byte aligned.
+ * b200_ln_modulate_e4m3: b200_ln_modulate's y (in fp32, before any 16-bit rounding) quantized per row -> out8 [rows, dim]
+ *   e4m3 bytes, row_scale [rows] fp32.  dim % 16 == 0.
+ * b200_linear_e4m3: out16[M, N] = epi(a_scale[row] * w_scale[col] * (A8[M, K] . W8[N, K]^T) + bias), epilogue
+ *   B200_EPI_BIAS or B200_EPI_BIAS_GELU, 16-bit output in `dtype`; K % 16 == 0 (else B200_ERR_UNSUPPORTED), N % 32 == 0;
+ *   A8, W8, out16, bias 16-byte aligned, w_scale 8-byte aligned.  Partial sums are kept in fp32 (DESIGN.md).            */
+B200_API int b200_quantize_rows_e4m3(const float* w, int rows, int cols, void* q8, float* scales, void* stream);
+B200_API int b200_ln_modulate_e4m3(const float* x, const float* shift, const float* scale, int64_t mod_batch_stride,
+                                   int rows_per_batch, void* out8, float* row_scale, int rows, int dim, void* stream);
+B200_API int b200_linear_e4m3(const void* A8, const float* a_scale, const void* W8, const float* w_scale, const float* bias, int M,
+                              int N, int K, int dtype, int epilogue, void* out16, void* stream);
 
 /* ---- training step (BASELINE config 5: train.py:206-222, fwd + bwd of models/latte.py under loss.backward()) -------------
  * The reference differentiates Latte.forward with torch autograd; the replacement keeps the same forward kernels, stores the

@@ -10,7 +10,7 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buffer
 OK = 0
 FP16, BF16 = 0, 1
@@ -28,7 +28,7 @@ class LatteShape(C.Structure):
 WEIGHT_FIELDS = (
     "patch_w", "patch_b", "pos_embed", "temp_embed", "t_w0", "t_b0", "t_w2", "t_b2", "y_table",
     "ada_w16", "ada_b", "qkv_w16", "qkv_b", "proj_w16", "proj_b", "fc1_w16", "fc1_b", "fc2_w16", "fc2_b",
-    "final_w", "final_b", "final_w16")
+    "final_w", "final_b", "final_w16", "qkv_w8", "qkv_ws", "fc1_w8", "fc1_ws")
 
 
 class LatteWeights(C.Structure):
@@ -123,6 +123,12 @@ EXPORTS = {
                                  C.c_int, C.c_void_p]),
     "b200_ln_modulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int,
                                    C.c_int, C.c_int, C.c_void_p]),
+    # FP8 (e4m3) sampling path
+    "b200_quantize_rows_e4m3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_ln_modulate_e4m3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                        C.c_int, C.c_void_p]),
+    "b200_linear_e4m3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                   C.c_int, C.c_void_p, C.c_void_p]),
     "b200_t2v_workspace_bytes": (C.c_size_t, [C.POINTER(T2VShape), C.c_int, C.c_int]),
     "b200_t2v_forward": (C.c_int, [C.POINTER(T2VShape), C.POINTER(T2VWeights), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

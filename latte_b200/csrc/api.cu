@@ -147,6 +147,13 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   const int bf16 = s->dtype == B200_BF16;
   const long long mod_bs = static_cast<long long>(depth) * 6 * D + 2 * D;
   const int HID = s->mlp_hidden;
+  B200_REQUIRE((!w->qkv_w8 || w->qkv_ws) && (!w->fc1_w8 || w->fc1_ws), B200_ERR_SHAPE, "e4m3 weights need their scales");
+  B200_REQUIRE((w->qkv_w8 || w->qkv_w16) && (w->fc1_w8 || w->fc1_w16), B200_ERR_SHAPE,
+               "qkv and fc1 need a 16-bit or an e4m3 weight copy");
+  // FP8 path: the e4m3 operand of QKV / fc1 and its row scales (T*D + 4T bytes) live in ws.h (T*D*2 bytes), which the GEMM
+  // consumes before attention or the next LayerNorm overwrites it
+  uint8_t* h8 = reinterpret_cast<uint8_t*>(ws.h);
+  float* h8_scale = reinterpret_cast<float*>(h8 + static_cast<size_t>(T) * D);
 
   // stream-K ordering flags: zero at the start of the step (every stream-K GEMM leaves them zero again; this memset only
   // makes the step independent of whatever the workspace held before -- a fresh allocation, an aborted run)
@@ -161,16 +168,21 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   // ---- blocks (latte.py:345-368); rows stay in (b, f, n) order for all of them
   for (int i = 0; i < depth; ++i) {
     const float* m = ws.mod + static_cast<size_t>(i) * 6 * D;  // [shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp]
-    const uint16_t* qkv_w = static_cast<const uint16_t*>(w->qkv_w16) + static_cast<size_t>(i) * 3 * D * D;
     const uint16_t* proj_w = static_cast<const uint16_t*>(w->proj_w16) + static_cast<size_t>(i) * D * D;
-    const uint16_t* fc1_w = static_cast<const uint16_t*>(w->fc1_w16) + static_cast<size_t>(i) * HID * D;
     const uint16_t* fc2_w = static_cast<const uint16_t*>(w->fc2_w16) + static_cast<size_t>(i) * D * HID;
 
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    GemmArgs ga{};
-    ga.A = ws.h; ga.W = qkv_w; ga.bias = w->qkv_b + static_cast<size_t>(i) * 3 * D;
-    ga.M = T; ga.N = 3 * D; ga.K = D; ga.bf16 = bf16; ga.epilogue = B200_EPI_BIAS; ga.out16 = ws.qkv; ga.w_const = 1;
-    B200_PROF(PROF_GEMM, launch_gemm(ga, stream));
+    if (w->qkv_w8) {
+      B200_PROF(PROF_LN, launch_ln_modulate_e4m3(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
+      B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w->qkv_w8) + static_cast<size_t>(i) * 3 * D * D,
+                                              w->qkv_ws + static_cast<size_t>(i) * 3 * D, w->qkv_b + static_cast<size_t>(i) * 3 * D,
+                                              T, 3 * D, D, bf16, B200_EPI_BIAS, ws.qkv, stream));
+    } else {
+      B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
+      GemmArgs ga{};
+      ga.A = ws.h; ga.W = static_cast<const uint16_t*>(w->qkv_w16) + static_cast<size_t>(i) * 3 * D * D; ga.bias = w->qkv_b + static_cast<size_t>(i) * 3 * D;
+      ga.M = T; ga.N = 3 * D; ga.K = D; ga.bf16 = bf16; ga.epilogue = B200_EPI_BIAS; ga.out16 = ws.qkv; ga.w_const = 1;
+      B200_PROF(PROF_GEMM, launch_gemm(ga, stream));
+    }
 
     AttnArgs aa{};
     aa.qkv = ws.qkv; aa.out = ws.h; aa.batch = batch; aa.frames = F; aa.tokens = N; aa.heads = H; aa.head_dim = hd;
@@ -183,11 +195,18 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
     gp.gate = m + 2 * D; gp.gate_batch_stride = mod_bs; gp.rows_per_batch = rows_per_batch; gp.sk_flags = ws.sk_flags;
     B200_PROF(PROF_GEMM, launch_gemm(gp, stream));
 
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    GemmArgs g1{};
-    g1.A = ws.h; g1.W = fc1_w; g1.bias = w->fc1_b + static_cast<size_t>(i) * HID;
-    g1.M = T; g1.N = HID; g1.K = D; g1.bf16 = bf16; g1.epilogue = B200_EPI_BIAS_GELU; g1.out16 = ws.g; g1.w_const = 1;
-    B200_PROF(PROF_GEMM, launch_gemm(g1, stream));
+    if (w->fc1_w8) {
+      B200_PROF(PROF_LN, launch_ln_modulate_e4m3(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
+      B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w->fc1_w8) + static_cast<size_t>(i) * HID * D,
+                                              w->fc1_ws + static_cast<size_t>(i) * HID, w->fc1_b + static_cast<size_t>(i) * HID,
+                                              T, HID, D, bf16, B200_EPI_BIAS_GELU, ws.g, stream));
+    } else {
+      B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
+      GemmArgs g1{};
+      g1.A = ws.h; g1.W = static_cast<const uint16_t*>(w->fc1_w16) + static_cast<size_t>(i) * HID * D; g1.bias = w->fc1_b + static_cast<size_t>(i) * HID;
+      g1.M = T; g1.N = HID; g1.K = D; g1.bf16 = bf16; g1.epilogue = B200_EPI_BIAS_GELU; g1.out16 = ws.g; g1.w_const = 1;
+      B200_PROF(PROF_GEMM, launch_gemm(g1, stream));
+    }
 
     GemmArgs g2{};
     g2.A = ws.g; g2.W = fc2_w; g2.bias = w->fc2_b + static_cast<size_t>(i) * D;
@@ -664,6 +683,23 @@ B200_API int b200_ln_modulate(const float* x, const float* shift, const float* s
   B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "dtype %d unknown", dtype);
   return b200::launch_ln_modulate(x, shift, scale, mod_batch_stride, rows_per_batch, out16, rows, dim,
                                   dtype == B200_BF16, static_cast<cudaStream_t>(stream));
+}
+
+B200_API int b200_quantize_rows_e4m3(const float* w, int rows, int cols, void* q8, float* scales, void* stream) {
+  return b200::launch_quantize_rows_e4m3(w, rows, cols, q8, scales, static_cast<cudaStream_t>(stream));
+}
+
+B200_API int b200_ln_modulate_e4m3(const float* x, const float* shift, const float* scale, int64_t mod_batch_stride,
+                                   int rows_per_batch, void* out8, float* row_scale, int rows, int dim, void* stream) {
+  return b200::launch_ln_modulate_e4m3(x, shift, scale, mod_batch_stride, rows_per_batch, out8, row_scale, rows, dim,
+                                       static_cast<cudaStream_t>(stream));
+}
+
+B200_API int b200_linear_e4m3(const void* A8, const float* a_scale, const void* W8, const float* w_scale, const float* bias, int M,
+                              int N, int K, int dtype, int epilogue, void* out16, void* stream) {
+  B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "dtype %d unknown", dtype);
+  return b200::launch_linear_e4m3(A8, a_scale, W8, w_scale, bias, M, N, K, dtype == B200_BF16, epilogue, out16,
+                                  static_cast<cudaStream_t>(stream));
 }
 
 // ---- training-step passes (train.cu) ----

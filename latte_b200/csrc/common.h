@@ -113,6 +113,10 @@ struct GemmArgs {
   int conv_dx[9], conv_dy[9], conv_dz[9];   // dz shifts the image index (temporal convolution over the frames of one clip)
 };
 int launch_gemm(const GemmArgs& a, cudaStream_t stream);
+// FP8 forward GEMM: out16[M, N] = epi(a_scale[row] * w_scale[col] * (A8[M, K] . W8[N, K]^T) + bias), both operands e4m3
+// K-major, epilogue B200_EPI_BIAS or B200_EPI_BIAS_GELU, K % 16 == 0 (16-byte rows), N % 32 == 0
+int launch_linear_e4m3(const void* A8, const float* a_scale, const void* W8, const float* w_scale, const float* bias, int M, int N,
+                       int K, int bf16, int epilogue, void* out16, cudaStream_t stream);
 
 struct AttnArgs {
   const void* qkv;   // [T, 3*heads*head_dim] 16-bit, row = token (b, f, n), cols [q | k | v] each [head][head_dim]
@@ -143,6 +147,11 @@ int launch_cross_attention(const CrossAttnArgs& a, cudaStream_t stream);
 
 int launch_ln_modulate(const float* x, const float* shift, const float* scale, long long mod_batch_stride,
                        int rows_per_batch, void* out16, int rows, int dim, int bf16, cudaStream_t stream);
+// the same LayerNorm + modulate quantized to e4m3 with one fp32 scale per row (out8 [rows, dim] bytes, row_scale [rows])
+int launch_ln_modulate_e4m3(const float* x, const float* shift, const float* scale, long long mod_batch_stride,
+                            int rows_per_batch, void* out8, float* row_scale, int rows, int dim, cudaStream_t stream);
+// per-row e4m3 quantization of an fp32 matrix [rows, cols]: scales[r] = amax(|row r|) / 448 (1 if zero), q = e4m3(w / s)
+int launch_quantize_rows_e4m3(const float* w, int rows, int cols, void* q8, float* scales, cudaStream_t stream);
 int launch_patch_embed(const float* x, int x_batch_mod, const float* w, const float* b, const float* pos, float* out,
                        int batch, int frames, int chans, int size, int patch, int dim, int channels_first, cudaStream_t stream);
 int launch_t2v_mod(const float* tables, const float* ts, const float* final_table, const float* emb, float* mod, int batch,

@@ -33,11 +33,16 @@ constexpr int LN_MAXV = 12;  // float4 per lane: dim <= 12*128 = 1536
 // consecutive rows and all warps are resident at once (register-limited to 32 warps/SM): a grid-stride loop left a
 // half-empty second wave.  The block's shift/scale vectors are staged in shared memory once, so the only global latency
 // on a row's critical path is the row itself.
-template <bool BF16, int NV>
+//
+// E4M3: the FP8 sampling path's instance.  The modulated fp32 row is quantized with one scale per row (token),
+// s = amax(|y|) / 448 (1 for an all-zero row), q = e4m3_rn_satfinite(y / s) with a correctly rounded division -- the
+// formula of quantize_rows_e4m3 -- and `out` receives dim bytes per row, row_scale[row] = s.  The amax is one more warp
+// reduction over the registers that already hold the row.
+template <bool BF16, int NV, bool E4M3 = false>
 __global__ void __launch_bounds__(128) ln_modulate_kernel(const float* __restrict__ x, const float* __restrict__ shift,
                                                           const float* __restrict__ scale, long long mod_bs,
                                                           int rows_per_batch, uint16_t* __restrict__ out, int rows,
-                                                          int dim, int rows_per_warp) {
+                                                          int dim, int rows_per_warp, float* __restrict__ row_scale) {
   extern __shared__ float4 s_mod[];  // [2][dim/4]: shift, scale of the batch row this block starts in
   const int lane = threadIdx.x & 31;
   const int nv = dim >> 2;
@@ -83,18 +88,47 @@ __global__ void __launch_bounds__(128) ln_modulate_kernel(const float* __restric
     const bool staged = b == b0;
     const float4* sh = reinterpret_cast<const float4*>(shift + b * mod_bs);
     const float4* sc = reinterpret_cast<const float4*>(scale + b * mod_bs);
-    uint2* orow = reinterpret_cast<uint2*>(out + static_cast<size_t>(row) * dim);
+    if constexpr (E4M3) {
+      // the modulated row replaces x in the registers (the next row is loaded after the stores)
+      float amax = 0.f;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int idx = lane + i * 32;
-      if (idx < nv) {
-        const float4 h = staged ? s_mod[idx] : __ldg(sh + idx);
-        const float4 c = staged ? s_mod[nv + idx] : __ldg(sc + idx);
-        const float y0 = fmaf((v[i].x - mean) * rstd, 1.0f + c.x, h.x);
-        const float y1 = fmaf((v[i].y - mean) * rstd, 1.0f + c.y, h.y);
-        const float y2 = fmaf((v[i].z - mean) * rstd, 1.0f + c.z, h.z);
-        const float y3 = fmaf((v[i].w - mean) * rstd, 1.0f + c.w, h.w);
-        orow[idx] = make_uint2(pack2<BF16>(y0, y1), pack2<BF16>(y2, y3));
+      for (int i = 0; i < NV; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nv) {
+          const float4 h = staged ? s_mod[idx] : __ldg(sh + idx);
+          const float4 c = staged ? s_mod[nv + idx] : __ldg(sc + idx);
+          v[i].x = fmaf((v[i].x - mean) * rstd, 1.0f + c.x, h.x);
+          v[i].y = fmaf((v[i].y - mean) * rstd, 1.0f + c.y, h.y);
+          v[i].z = fmaf((v[i].z - mean) * rstd, 1.0f + c.z, h.z);
+          v[i].w = fmaf((v[i].w - mean) * rstd, 1.0f + c.w, h.w);
+          amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+      const float s = e4m3_scale(amax);
+      uint32_t* orow = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(out) + static_cast<size_t>(row) * dim);
+#pragma unroll
+      for (int i = 0; i < NV; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nv)
+          orow[idx] = pack_e4m3x4(__fdiv_rn(v[i].x, s), __fdiv_rn(v[i].y, s), __fdiv_rn(v[i].z, s), __fdiv_rn(v[i].w, s));
+      }
+      if (lane == 0) row_scale[row] = s;
+    } else {
+      uint2* orow = reinterpret_cast<uint2*>(out + static_cast<size_t>(row) * dim);
+#pragma unroll
+      for (int i = 0; i < NV; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nv) {
+          const float4 h = staged ? s_mod[idx] : __ldg(sh + idx);
+          const float4 c = staged ? s_mod[nv + idx] : __ldg(sc + idx);
+          const float y0 = fmaf((v[i].x - mean) * rstd, 1.0f + c.x, h.x);
+          const float y1 = fmaf((v[i].y - mean) * rstd, 1.0f + c.y, h.y);
+          const float y2 = fmaf((v[i].z - mean) * rstd, 1.0f + c.z, h.z);
+          const float y3 = fmaf((v[i].w - mean) * rstd, 1.0f + c.w, h.w);
+          orow[idx] = make_uint2(pack2<BF16>(y0, y1), pack2<BF16>(y2, y3));
+        }
       }
     }
     if (rr + 1 < rows_per_warp && row + 1 < rows) {
@@ -106,10 +140,10 @@ __global__ void __launch_bounds__(128) ln_modulate_kernel(const float* __restric
   }
 }
 
-template <bool BF16, int NV>
+template <bool BF16, int NV, bool E4M3 = false>
 int ln_launch(cudaStream_t stream, const float* x, const float* shift, const float* scale, long long mod_bs, int rpb,
-              uint16_t* out, int rows, int dim, int sms) {
-  auto kern = ln_modulate_kernel<BF16, NV>;
+              uint16_t* out, int rows, int dim, int sms, float* row_scale = nullptr) {
+  auto kern = ln_modulate_kernel<BF16, NV, E4M3>;
   const size_t smem = static_cast<size_t>(dim) * 2 * sizeof(float);
   static int blocks_per_sm_dev[64] = {};   // per instantiation and device: what the register/smem footprint really allows
   int dev = 0;
@@ -125,7 +159,8 @@ int ln_launch(cudaStream_t stream, const float* x, const float* shift, const flo
   const int resident_warps = sms * blocks_per_sm * wpb;
   const int rpw = (rows + resident_warps - 1) / resident_warps;
   const int blocks = (rows + wpb * rpw - 1) / (wpb * rpw);
-  B200_CHECK_CUDA(launch_pdl(kern, dim3(blocks), dim3(128), smem, stream, x, shift, scale, mod_bs, rpb, out, rows, dim, rpw));
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(blocks), dim3(128), smem, stream, x, shift, scale, mod_bs, rpb, out, rows, dim, rpw,
+                                    row_scale));
   return B200_OK;
 }
 
@@ -136,6 +171,43 @@ int ln_dispatch(int nvmax, cudaStream_t stream, const float* x, const float* shi
   if (nvmax <= 6) return ln_launch<BF16, 6>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms);
   if (nvmax <= 9) return ln_launch<BF16, 9>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms);
   return ln_launch<BF16, LN_MAXV>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms);
+}
+
+// the e4m3 instances (the operand type of the 16-bit template argument does not matter: one instance per width)
+int ln_dispatch_e4m3(int nvmax, cudaStream_t stream, const float* x, const float* shift, const float* scale, long long mod_bs,
+                     int rpb, uint8_t* out8, float* row_scale, int rows, int dim, int sms) {
+  uint16_t* out = reinterpret_cast<uint16_t*>(out8);
+  if (nvmax <= 3) return ln_launch<false, 3, true>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms, row_scale);
+  if (nvmax <= 6) return ln_launch<false, 6, true>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms, row_scale);
+  if (nvmax <= 9) return ln_launch<false, 9, true>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms, row_scale);
+  return ln_launch<false, LN_MAXV, true>(stream, x, shift, scale, mod_bs, rpb, out, rows, dim, sms, row_scale);
+}
+
+// ---------------------------------------------------------------------------------- quantize_rows_e4m3
+// One warp per row of an fp32 matrix [rows, cols] (a weight W[N, K]: one scale per output channel): s = amax(|row|) / 448
+// (1 for an all-zero row), q = e4m3_rn_satfinite(w / s), the division correctly rounded.  Two passes over the row in
+// global memory: this runs once per weight packing, not per step.
+__global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const float* __restrict__ w, int rows, int cols,
+                                                                 uint32_t* __restrict__ q, float* __restrict__ scales) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const float4* wr = reinterpret_cast<const float4*>(w + static_cast<size_t>(row) * cols);
+  const int n4 = cols >> 2;
+  float amax = 0.f;
+  for (int i = lane; i < n4; i += 32) {
+    const float4 v = __ldg(wr + i);
+    amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float s = e4m3_scale(amax);
+  uint32_t* qr = q + static_cast<size_t>(row) * n4;
+  for (int i = lane; i < n4; i += 32) {
+    const float4 v = __ldg(wr + i);
+    qr[i] = pack_e4m3x4(__fdiv_rn(v.x, s), __fdiv_rn(v.y, s), __fdiv_rn(v.z, s), __fdiv_rn(v.w, s));
+  }
+  if (lane == 0) scales[row] = s;
 }
 
 // ---------------------------------------------------------------------------------- patch_embed
@@ -589,6 +661,32 @@ int launch_ln_modulate(const float* x, const float* shift, const float* scale, l
   uint16_t* o = reinterpret_cast<uint16_t*>(out16);
   if (bf16) return ln_dispatch<true>(nvmax, stream, x, shift, scale, mod_batch_stride, rows_per_batch, o, rows, dim, sms);
   return ln_dispatch<false>(nvmax, stream, x, shift, scale, mod_batch_stride, rows_per_batch, o, rows, dim, sms);
+}
+
+int launch_ln_modulate_e4m3(const float* x, const float* shift, const float* scale, long long mod_batch_stride,
+                            int rows_per_batch, void* out8, float* row_scale, int rows, int dim, cudaStream_t stream) {
+  B200_REQUIRE(rows > 0 && dim > 0 && dim % 16 == 0 && dim <= LN_MAXV * 128, B200_ERR_SHAPE,
+               "ln_modulate_e4m3: dim %d must be a multiple of 16 and <= %d", dim, LN_MAXV * 128);
+  B200_REQUIRE(rows_per_batch > 0 && mod_batch_stride % 4 == 0, B200_ERR_SHAPE, "ln_modulate_e4m3: bad batch geometry");
+  B200_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(shift) | reinterpret_cast<uintptr_t>(scale) |
+                 reinterpret_cast<uintptr_t>(out8)) & 15) == 0 && row_scale && (reinterpret_cast<uintptr_t>(row_scale) & 3) == 0,
+               B200_ERR_ALIGN, "ln_modulate_e4m3: x, shift, scale, out must be 16-byte aligned, row_scale 4-byte");
+  int sms = 0;
+  B200_TRY(device_sm_count(&sms));
+  return ln_dispatch_e4m3((dim / 4 + 31) / 32, stream, x, shift, scale, mod_batch_stride, rows_per_batch,
+                          static_cast<uint8_t*>(out8), row_scale, rows, dim, sms);
+}
+
+int launch_quantize_rows_e4m3(const float* w, int rows, int cols, void* q8, float* scales, cudaStream_t stream) {
+  B200_REQUIRE(rows > 0 && cols > 0, B200_ERR_SHAPE, "quantize_rows_e4m3: bad shape %d x %d", rows, cols);
+  B200_REQUIRE(cols % 16 == 0, B200_ERR_UNSUPPORTED, "quantize_rows_e4m3: cols %d must be a multiple of 16 (16-byte rows)", cols);
+  B200_REQUIRE(((reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(q8)) & 15) == 0 && scales &&
+                   (reinterpret_cast<uintptr_t>(scales) & 3) == 0,
+               B200_ERR_ALIGN, "quantize_rows_e4m3: w and q must be 16-byte aligned, scales 4-byte");
+  const int blocks = (rows + 7) / 8;
+  quantize_rows_e4m3_kernel<<<blocks, 256, 0, stream>>>(w, rows, cols, static_cast<uint32_t*>(q8), scales);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return B200_OK;
 }
 
 int launch_patch_embed(const float* x, int x_batch_mod, const float* w, const float* b, const float* pos, float* out,

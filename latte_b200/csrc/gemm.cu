@@ -531,6 +531,204 @@ GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool s
   return g;
 }
 
+// ---------------------------------------------------------------------------------------------------- FP8 (e4m3) GEMM
+// out16 = epi(s_a[row] * s_w[col] * (A8 . W8^T) + bias) for QKV and fc1 of the sampling forward: A8 and s_a come from
+// the e4m3 instance of ln_modulate (one scale per token), W8 and s_w from quantize_rows_e4m3 (one per output channel).
+// The mainloop is gemm_kernel's with K-major operands: CTA pairs, the multicast W half, 128B swizzle, the TMA producer
+// warpgroup.  A 128-byte swizzle row now holds 128 elements, so one stage is one 128-wide k-block with the same bytes as a
+// 16-bit stage, and a k-block is four m64nNk32 e4m3 wgmma whose descriptors advance 32 bytes each, as the 16-bit k16 steps
+// do.  K need not be a multiple of 128: the last k-block's columns past K are zero-filled by TMA (which still counts the
+// whole box toward the barrier's bytes).
+// Accumulation: FP8 wgmma keeps fewer accumulator bits than fp32 (DESIGN.md §6, FP8 sampling path), so each k-block is
+// summed in registers of its own -- alternately acc0 and acc1, the k-block's first wgmma overwriting -- and added into the
+// fp32 total `sum` once the NEXT k-block's wgmma are in flight: the k-loop still waits with wgmma_wait<1>.  The three
+// 64-float fragments fit the consumers' 232 registers at BN = 128 only, so that is the one tile width.
+constexpr int BN8 = 128;
+constexpr int BK8 = 128;
+
+template <int EPI, bool BF16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+fp8_linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const GemmDev p, const float* __restrict__ a_scale,
+                  const float* __restrict__ w_scale) {
+  using C = Cfg<BN8, EPI>;
+  static_assert(C::A_BYTES == BM * BK8 && C::B_BYTES == BN8 * BK8, "a stage holds one e4m3 k-block");
+  static_assert(EPI == B200_EPI_BIAS || EPI == B200_EPI_BIAS_GELU, "16-bit output epilogues only");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + C::STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmC);
+    for (int i = 0; i < C::STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 4);
+    }
+    fence_mbar_init();
+  }
+  cluster_sync_all();
+  pdl_launch_dependents();
+
+  const uint32_t rank = cluster_ctarank();
+  const int num_pair_m = (p.num_m + 1) / 2;
+  const int num_tiles = num_pair_m * p.num_n;
+  const int my_pair = blockIdx.x >> 1;
+  const int num_pairs = gridDim.x >> 1;
+  const int num_kb = (p.K + BK8 - 1) / BK8;
+
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (as gemm_kernel's)
+    setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) {
+      pdl_wait();
+      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, false);
+      int stage = 0;
+      uint32_t phase = 0;
+      int tile, kb0, kb1;
+      while (sched.next(tile, kb0, kb1)) {
+        const int m_blk = 2 * (tile / p.num_n) + static_cast<int>(rank), n_blk = tile % p.num_n;
+        const int w_row0 = n_blk * BN8 + static_cast<int>(rank) * (BN8 / 2);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
+          uint8_t* sa = smem + stage * C::STAGE_BYTES;
+          tma_load_2d(sa, &tmA, &full[stage], kb * BK8, m_blk * BM);
+          tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK8, w_row0, 0x3);
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else {
+    // ------------------------------------------------------------------ MMA + epilogue: warpgroups 1, 2 (64 rows each)
+    setmaxnreg_inc<kConsumerRegs>();
+    pdl_wait();
+    const int wg = (warp >> 2) - 1;
+    const int te = threadIdx.x & 127;
+    const int w4 = te >> 5, g = lane >> 2, cq = lane & 3;
+    const uint32_t empty_peer = mapa_u32(&empty[0], rank ^ 1u);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc0[BN8 / 2], acc1[BN8 / 2], sum[BN8 / 2];
+    uint8_t* epi = smem + C::EPI_OFF;
+    int ep = 0;
+    int prev = -1;                            // slot of the k-block whose wgmma may still be running
+    // one k-block into `cur`; once the previous k-block's wgmma have completed, its slot is released in both CTAs and its
+    // partial sum `done` is added into `sum`
+    auto kblock = [&](float (&cur)[BN8 / 2], float (&done)[BN8 / 2]) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES), sb = sa + C::A_BYTES;
+      wgmma_fence();
+      const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128);
+      const uint64_t db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
+#pragma unroll
+      for (int k = 0; k < BK8 / 32; ++k)
+        WgmmaE4M3<BN8>::mma(cur, gmma_desc_advance(da, k * 32), gmma_desc_advance(db, k * 32), k ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      reg_fence(done);
+      if (prev >= 0 && te == 0) {
+        mbar_arrive(&empty[prev]);
+        mbar_arrive_cluster(empty_peer + prev * 8);
+      }
+      prev = stage;
+      if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+#pragma unroll
+      for (int i = 0; i < BN8 / 2; ++i) sum[i] += done[i];
+    };
+    auto drain = [&](float (&cur)[BN8 / 2]) {
+      wgmma_wait<0>();
+      reg_fence(cur);
+      if (te == 0) {
+        mbar_arrive(&empty[prev]);
+        mbar_arrive_cluster(empty_peer + prev * 8);
+      }
+#pragma unroll
+      for (int i = 0; i < BN8 / 2; ++i) sum[i] += cur[i];
+    };
+    TileSched sched(my_pair, num_pairs, num_tiles, num_kb, false);
+    int tile, kb0, kb1;
+    while (sched.next(tile, kb0, kb1)) {
+      const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN8;
+      prev = -1;                              // the previous tile's last slot was released by its drain
+#pragma unroll
+      for (int i = 0; i < BN8 / 2; ++i) { sum[i] = 0.f; acc1[i] = 0.f; }
+      for (int kb = kb0;;) {                  // k-blocks alternate between acc0 and acc1 (acc1 = 0 before the first)
+        kblock(acc0, acc1);
+        if (++kb == kb1) { drain(acc0); break; }
+        kblock(acc1, acc0);
+        if (++kb == kb1) { drain(acc1); break; }
+      }
+
+      // the 16-bit epilogue of gemm_kernel: v = (sum * s_a[row]) * s_w[col] + bias (each step rounded), then GELU for fc1
+      const int m0w = m0 + wg * 64;
+      const int lr0 = w4 * 16 + g;
+      float sa_row[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = m0w + lr0 + 8 * h;
+        sa_row[h] = row < p.M ? __ldg(a_scale + row) : 0.f;   // rows past M are clipped by the TMA store
+      }
+      const int mi = lane >> 3;
+      const int lrow = w4 * 16 + (lane & 7) + 8 * (mi & 1);
+#pragma unroll
+      for (int c = 0; c < BN8 / 64; ++c) {
+        if (n0 + 64 * c >= p.N) break;
+        uint8_t* buf = epi + (2 * wg + (ep & 1)) * kEpiBufBytes;
+        const uint32_t row_addr = smem_u32(buf) + lrow * 128;
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {
+          uint32_t v[4];
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            const int j = 8 * c + 2 * jp + q, col = n0 + 8 * j + 2 * cq;
+            const bool col_ok = col < p.N;
+            const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+            const float2 s2 = col_ok ? __ldg(reinterpret_cast<const float2*>(w_scale + col)) : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float f0 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h], sa_row[h]), s2.x), b2.x);
+              float f1 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h + 1], sa_row[h]), s2.y), b2.y);
+              if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+              v[2 * q + h] = pack2<BF16>(f0, f1);
+            }
+          }
+          const uint32_t unit = ((2 * jp + (mi >> 1)) ^ (lane & 7)) << 4;
+          stmatrix_x4(row_addr + unit, v[0], v[1], v[2], v[3]);
+        }
+        fence_proxy_async_smem();
+        epi_bar(wg);
+        if (te == 0) {
+          tma_store_2d(&tmC, buf, n0 + 64 * c, m0w);
+          tma_store_commit();
+          tma_store_wait_read<1>();
+        }
+        epi_bar(wg);
+        ++ep;
+      }
+    }
+    if (te == 0) tma_store_wait_all<0>();
+  }
+
+  cluster_sync_all();
+}
+
+template <int EPI, bool BF16>
+int launch_e4m3(const GemmMaps& tm, const GemmDev& p, const float* a_scale, const float* w_scale, int grid, cudaStream_t stream) {
+  using C = Cfg<BN8, EPI>;
+  auto kern = fp8_linear_kernel<EPI, BF16>;
+  B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tm.a, tm.b, tm.c, p, a_scale, w_scale));
+  return B200_OK;
+}
+
 }  // namespace
 
 int gemm_schedule(int M, int N, int K, int epilogue, int block_n, int sms, int* bn_out, int* pairs_out, int* streamk_out,
@@ -701,6 +899,51 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     case 192: return launch_bn<192>(a.bf16, a.epilogue, a.mn_major, tm, p, grid, stream);
     default: return launch_bn<256>(a.bf16, a.epilogue, a.mn_major, tm, p, grid, stream);
   }
+}
+
+int launch_linear_e4m3(const void* A8, const float* a_scale, const void* W8, const float* w_scale, const float* bias, int M, int N,
+                       int K, int bf16, int epilogue, void* out16, cudaStream_t stream) {
+  B200_REQUIRE(M > 0 && N > 0 && K > 0, B200_ERR_SHAPE, "gemm e4m3: bad shape M=%d N=%d K=%d", M, N, K);
+  B200_REQUIRE(K % 16 == 0, B200_ERR_UNSUPPORTED, "gemm e4m3: K=%d: rows must be a multiple of 16 bytes", K);
+  B200_REQUIRE(N % 32 == 0, B200_ERR_SHAPE, "gemm e4m3: N=%d must be a multiple of 32", N);
+  B200_REQUIRE(epilogue == B200_EPI_BIAS || epilogue == B200_EPI_BIAS_GELU, B200_ERR_UNSUPPORTED,
+               "gemm e4m3: epilogue %d not built (bias and bias+GELU only)", epilogue);
+  B200_REQUIRE(((reinterpret_cast<uintptr_t>(A8) | reinterpret_cast<uintptr_t>(W8) | reinterpret_cast<uintptr_t>(out16) |
+                 reinterpret_cast<uintptr_t>(bias)) & 15) == 0 && A8 && W8 && out16,
+               B200_ERR_ALIGN, "gemm e4m3: A, W, out16 (and bias) must be 16-byte aligned");
+  B200_REQUIRE(a_scale && w_scale && (reinterpret_cast<uintptr_t>(a_scale) & 3) == 0 && (reinterpret_cast<uintptr_t>(w_scale) & 7) == 0,
+               B200_ERR_ALIGN, "gemm e4m3: a_scale (4-byte) and w_scale (8-byte aligned) are required");
+  B200_TRY(check_arch());
+  int sms = 0;
+  B200_TRY(device_sm_count(&sms));
+  const GemmPlan plan = plan_gemm(M, N, K, false, BN8, sms);
+  GemmMaps tm;
+  {
+    const uint64_t dimsA[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(M)};
+    const uint64_t strA[1] = {static_cast<uint64_t>(K)};
+    const uint32_t boxA[2] = {BK8, BM};
+    B200_TRY(make_tmap(&tm.a, A8, 1, 2, dimsA, strA, boxA, TMAP_SW_128));
+    const uint64_t dimsB[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
+    const uint32_t boxB[2] = {BK8, BN8 / 2};
+    B200_TRY(make_tmap(&tm.b, W8, 1, 2, dimsB, strA, boxB, TMAP_SW_128));
+    const uint64_t dimsC[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(M)};
+    const uint64_t strC[1] = {static_cast<uint64_t>(N) * 2};
+    const uint32_t boxC[2] = {64, 64};
+    B200_TRY(make_tmap_16bit(&tm.c, out16, 2, dimsC, strC, boxC, TMAP_SW_128));
+  }
+  GemmDev p{};
+  p.M = M; p.N = N; p.K = K;
+  p.num_m = (M + BM - 1) / BM;
+  p.num_n = (N + BN8 - 1) / BN8;
+  p.bias = bias;
+  p.out16 = out16;
+  p.rows_per_batch = 1;
+  const int grid = 2 * plan.pairs;
+  if (epilogue == B200_EPI_BIAS)
+    return bf16 ? launch_e4m3<B200_EPI_BIAS, true>(tm, p, a_scale, w_scale, grid, stream)
+                : launch_e4m3<B200_EPI_BIAS, false>(tm, p, a_scale, w_scale, grid, stream);
+  return bf16 ? launch_e4m3<B200_EPI_BIAS_GELU, true>(tm, p, a_scale, w_scale, grid, stream)
+              : launch_e4m3<B200_EPI_BIAS_GELU, false>(tm, p, a_scale, w_scale, grid, stream);
 }
 
 }  // namespace b200

@@ -270,4 +270,16 @@ __device__ __forceinline__ float2 unpack2(uint32_t u) {
   }
 }
 
+// ----------------------------------------------------------------------------- e4m3 packing
+// four fp32 values -> four e4m3 bytes, a in the lowest: round to nearest even, saturating to +-448 (cvt puts its first
+// source operand in the upper byte of each pair)
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+  uint16_t lo, hi;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
+  return static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+}
+// the per-row scale of an e4m3 operand: amax / 448 (448 = the largest finite e4m3), 1 for an all-zero row
+__device__ __forceinline__ float e4m3_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f; }
+
 }  // namespace b200

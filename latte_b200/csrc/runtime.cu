@@ -114,10 +114,12 @@ int encode_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, co
     case TMAP_SW_128: s = CU_TENSOR_MAP_SWIZZLE_128B; break;
     default: break;
   }
-  // the bit pattern is moved, never interpreted, so one unsigned type per element size serves fp16/bf16 and fp32
-  B200_REQUIRE(elem_bytes == 2 || elem_bytes == 4, B200_ERR_DTYPE, "tensor map element size %d unsupported", elem_bytes);
+  // the bit pattern is moved, never interpreted, so one unsigned type per element size serves e4m3, fp16/bf16 and fp32
+  B200_REQUIRE(elem_bytes == 1 || elem_bytes == 2 || elem_bytes == 4, B200_ERR_DTYPE, "tensor map element size %d unsupported", elem_bytes);
   // 4-byte maps are typed FLOAT32 so that TMA reductions (cp.reduce ... .add) add floats
-  const CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const CUtensorMapDataType dt = elem_bytes == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                 : elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16
+                                                   : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = fn(out, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
                   gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, s, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

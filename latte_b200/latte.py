@@ -157,6 +157,10 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         #: eval-mode calls replay a CUDA graph of the whole forward (captured per (batch, cfg) signature on its second
         #: use; results are bit-identical to the eager launch sequence).  Set False to always launch eagerly.
         self.use_cuda_graphs = True
+        #: sampling runs QKV and fc1 -- the two GEMMs fed by LayerNorm + modulate -- with FP8 (e4m3) tensor-core operands:
+        #: per-token activation scales, per-output-channel weight scales, fp32 accumulation.  Every other operand keeps the
+        #: 16-bit type.  Eval / no-grad calls only; a training forward raises.  Toggling it repacks the weights.
+        self.use_fp8 = False
         #: training steps keep each block's input only and rerun the block in the backward (`enable_gradient_checkpointing`)
         self.gradient_checkpointing = False
 
@@ -206,7 +210,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         ver = 0
         for p in self.parameters():
             ver += p._version
-        return (ver, w0.data_ptr(), w0.device, w0.dtype, self.compute_dtype)
+        return (ver, w0.data_ptr(), w0.device, w0.dtype, self.compute_dtype, bool(self.use_fp8))
 
     def repack(self):
         """Drop the packed operand cache (call after mutating parameters through `.data`)."""
@@ -218,6 +222,12 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
     @torch.no_grad()
     def _pack(self):
         if self._frozen is not None:          # inside a sampling loop (precompute_conditioning .. clear_conditioning)
+            if (self._frozen[2].get("qkv_w8") is not None) == bool(self.use_fp8):
+                return self._frozen
+            # use_fp8 was toggled inside the loop: pack in the new mode (the precomputed conditioning rows do not depend on
+            # it) and keep that packing for the rest of the loop
+            self._frozen = None
+            self._frozen = self._pack()
             return self._frozen
         key = self._pack_key()
         if self._packed is not None and key == self._packed_key:
@@ -243,17 +253,34 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         T["ada_w16"] = torch.cat([b.adaLN_modulation[1].weight.detach() for b in blocks] +
                                  [self.final_layer.adaLN_modulation[1].weight.detach()]).to(device=dev, dtype=od).contiguous()
         T["ada_b"] = cat32([b.adaLN_modulation[1].bias for b in blocks] + [self.final_layer.adaLN_modulation[1].bias])
-        T["qkv_w16"] = stack16([b.attn.qkv.weight for b in blocks])
+        # with use_fp8 the forward reads only the e4m3 copies of QKV and fc1 (below), so no 16-bit ones are made
+        T["qkv_w16"] = None if self.use_fp8 else stack16([b.attn.qkv.weight for b in blocks])
         T["qkv_b"] = cat32([b.attn.qkv.bias for b in blocks])
         T["proj_w16"] = stack16([b.attn.proj.weight for b in blocks])
         T["proj_b"] = cat32([b.attn.proj.bias for b in blocks])
-        T["fc1_w16"] = stack16([b.mlp.fc1.weight for b in blocks])
+        T["fc1_w16"] = None if self.use_fp8 else stack16([b.mlp.fc1.weight for b in blocks])
         T["fc1_b"] = cat32([b.mlp.fc1.bias for b in blocks])
         T["fc2_w16"] = stack16([b.mlp.fc2.weight for b in blocks])
         T["fc2_b"] = cat32([b.mlp.fc2.bias for b in blocks])
         T["final_w"] = f32(self.final_layer.linear.weight)
         T["final_b"] = f32(self.final_layer.linear.bias)
         T["final_w16"] = self.final_layer.linear.weight.detach().to(device=dev, dtype=od).contiguous()
+        for name in ("qkv_w8", "qkv_ws", "fc1_w8", "fc1_ws"):
+            T[name] = None
+        if self.use_fp8:
+            # ONE quantization call for every QKV and fc1 weight (the same width D): rows [0, depth*3D) are QKV, stacked over
+            # blocks like the 16-bit copies, then fc1; one scale per output channel (b200_quantize_rows_e4m3)
+            w32 = torch.cat([b.attn.qkv.weight.detach() for b in blocks] + [b.mlp.fc1.weight.detach() for b in blocks]).to(
+                device=dev, dtype=torch.float32).contiguous()
+            rows, nq = w32.shape[0], self.depth * 3 * D
+            q8 = torch.empty(rows, D, dtype=torch.uint8, device=dev)
+            ws8 = torch.empty(rows, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                rc = _lib.load().b200_quantize_rows_e4m3(w32.data_ptr(), rows, D, q8.data_ptr(), ws8.data_ptr(),
+                                                         torch.cuda.current_stream(dev).cuda_stream)
+            _lib.check(rc, "b200_quantize_rows_e4m3")
+            T["qkv_w8"], T["fc1_w8"] = q8[:nq], q8[nq:]
+            T["qkv_ws"], T["fc1_ws"] = ws8[:nq], ws8[nq:]
 
         w = _lib.LatteWeights()
         for name in _lib.WEIGHT_FIELDS:
@@ -336,6 +363,8 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         `torch.autocast(bfloat16)` / fp32 parameters (the reference's mixed-precision recipe) or the parameter dtype if that is
         16-bit; accumulation, the residual stream, LayerNorm statistics and every gradient buffer are fp32."""
         from . import training
+        if self.use_fp8:
+            raise NotImplementedError("latte_b200: FP8 is a sampling path; clear use_fp8 to train")
         if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[2] != self.in_channels \
                 or x.shape[3] != self.input_size or x.shape[4] != self.input_size:
             raise ValueError(f"x must be (B, {self.num_frames}, {self.in_channels}, {self.input_size}, {self.input_size}), got {tuple(x.shape)}")
@@ -375,7 +404,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         state, so its launch sequence can be captured once per call signature and replayed with the inputs copied into
         fixed buffers: the per-step host cost drops from ~200 launches to three small copies and one graph launch.
         First use of a signature runs eagerly (it also sets per-device kernel attributes), the second captures."""
-        key = (B, bool(use_cfg), float(cfg_scale), yy is not None, mod is not None, dev)
+        key = (B, bool(use_cfg), float(cfg_scale), yy is not None, mod is not None, dev, bool(self.use_fp8))
         if self._graphs is None:
             self._graphs = {}
         st = self._graphs.get(key)

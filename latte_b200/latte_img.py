@@ -37,6 +37,10 @@ class LatteIMG(Latte):
             return super().forward(x, t, y, text_embedding=text_embedding, use_fp16=use_fp16, trajectory_step=trajectory_step)
         if text_embedding is not None:
             raise NotImplementedError("text_embedding (extras=78) is outside the built hot path")
+        if self.use_fp8:
+            # frames with images run the training engine's 16-bit forward (training and eval alike): no silent fallback
+            raise NotImplementedError("latte_b200: FP8 is a sampling path of the video forward; LatteIMG with images "
+                                      "(use_image_num > 0) has none -- clear use_fp8")
         if trajectory_step is not None:
             raise ValueError("latte_b200: trajectory conditioning is a sampling path; it takes no images (use_image_num = 0)")
         if I < 0:

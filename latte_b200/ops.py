@@ -96,6 +96,51 @@ def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, rows_
     return out
 
 
+def quantize_rows_e4m3(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """w fp32 [rows, cols] -> (q [rows, cols] float8_e4m3fn, scales fp32 [rows]): s = amax(|row|) / 448 (1 for a zero row),
+    q = e4m3_rn_satfinite(row / s) (b200_quantize_rows_e4m3)."""
+    _need_cuda(w)
+    assert w.dtype == torch.float32 and w.dim() == 2 and w.is_contiguous()
+    q = torch.empty(w.shape, dtype=torch.uint8, device=w.device)
+    s = torch.empty(w.shape[0], dtype=torch.float32, device=w.device)
+    with torch.cuda.device(w.device):
+        rc = _lib.load().b200_quantize_rows_e4m3(w.data_ptr(), w.shape[0], w.shape[1], q.data_ptr(), s.data_ptr(), _stream(w))
+    _lib.check(rc, "b200_quantize_rows_e4m3")
+    return q.view(torch.float8_e4m3fn), s
+
+
+def ln_modulate_e4m3(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor,
+                     rows_per_batch: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """ln_modulate quantized per row: x fp32 [rows, D] -> (q [rows, D] float8_e4m3fn, row scales fp32 [rows])."""
+    _need_cuda(x, shift, scale)
+    assert x.dtype == torch.float32 and x.is_contiguous() and shift.stride(0) == scale.stride(0)
+    q = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
+    s = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        rc = _lib.load().b200_ln_modulate_e4m3(x.data_ptr(), shift.data_ptr(), scale.data_ptr(), shift.stride(0), rows_per_batch,
+                                               q.data_ptr(), s.data_ptr(), x.shape[0], x.shape[1], _stream(x))
+    _lib.check(rc, "b200_ln_modulate_e4m3")
+    return q.view(torch.float8_e4m3fn), s
+
+
+def linear_e4m3(a8: torch.Tensor, a_scale: torch.Tensor, w8: torch.Tensor, w_scale: torch.Tensor,
+                bias: torch.Tensor | None = None, gelu: bool = False, dtype: torch.dtype = torch.float16) -> torch.Tensor:
+    """out16 = (gelu_tanh)(a_scale[:, None] * w_scale[None, :] * (a8 @ w8.T) + bias) in `dtype`; a8 [M, K], w8 [N, K] e4m3
+    (float8_e4m3fn or its uint8 bytes), scales and bias fp32 (b200_linear_e4m3)."""
+    _need_cuda(a8, a_scale, w8, w_scale, bias)
+    assert a8.element_size() == 1 and w8.element_size() == 1 and a8.is_contiguous() and w8.is_contiguous()
+    assert a_scale.dtype == w_scale.dtype == torch.float32 and a_scale.is_contiguous() and w_scale.is_contiguous()
+    M, K = a8.shape
+    N = w8.shape[0]
+    out = torch.empty(M, N, dtype=dtype, device=a8.device)
+    with torch.cuda.device(a8.device):
+        rc = _lib.load().b200_linear_e4m3(a8.data_ptr(), a_scale.data_ptr(), w8.data_ptr(), w_scale.data_ptr(),
+                                          bias.data_ptr() if bias is not None else None, M, N, K, _dt(out),
+                                          _lib.EPI_BIAS_GELU if gelu else _lib.EPI_BIAS, out.data_ptr(), _stream(a8))
+    _lib.check(rc, "b200_linear_e4m3")
+    return out
+
+
 def cross_attention(q: torch.Tensor, kv: torch.Tensor, batch: int, q_rows_per_batch: int, kv_len: int, heads: int,
                     key_bias: torch.Tensor | None = None) -> torch.Tensor:
     """q [batch*q_rows, heads*hd] 16-bit; kv [batch*kv_len, 2*heads*hd] 16-bit ([k | v]); kv_len <= 128 -> out like q.
