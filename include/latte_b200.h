@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 5
+#define B200_ABI_VERSION 6
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
 #else
@@ -131,7 +131,7 @@ typedef struct B200T2VWeights {
   const float* cap_b2;
   const float* tables;     /* scale_shift_table of every block in execution order s0,t0,s1,t1,...: [2*layers][6][D] */
   const float* final_table;/* scale_shift_table [2][D] */
-  const void* s_qkv_w16;   /* transformer_blocks.l.attn1.to_q|to_k|to_v.weight stacked [l][3D, D] */
+  const void* s_qkv_w16;   /* transformer_blocks.l.attn1.to_q|to_k|to_v.weight stacked [l][3D, D] (NULL allowed when s_qkv_w8 is set) */
   const float* s_qkv_b;
   const void* s_out_w16;   /* ...attn1.to_out.0.weight [l][D, D] */
   const float* s_out_b;
@@ -141,21 +141,34 @@ typedef struct B200T2VWeights {
   const float* c_kv_b;
   const void* c_out_w16;   /* ...attn2.to_out.0.weight [l][D, D] */
   const float* c_out_b;
-  const void* s_fc1_w16;   /* ...ff.net.0.proj.weight [l][4D, D] */
+  const void* s_fc1_w16;   /* ...ff.net.0.proj.weight [l][4D, D] (NULL allowed when s_fc1_w8 is set) */
   const float* s_fc1_b;
   const void* s_fc2_w16;   /* ...ff.net.2.weight [l][D, 4D] */
   const float* s_fc2_b;
-  const void* t_qkv_w16;   /* temporal_transformer_blocks.l.attn1 ... */
+  const void* t_qkv_w16;   /* temporal_transformer_blocks.l.attn1 ... (NULL allowed when t_qkv_w8 is set) */
   const float* t_qkv_b;
   const void* t_out_w16;
   const float* t_out_b;
-  const void* t_fc1_w16;
+  const void* t_fc1_w16;   /* (NULL allowed when t_fc1_w8 is set) */
   const float* t_fc1_b;
   const void* t_fc2_w16;
   const float* t_fc2_b;
   const float* final_w;    /* proj_out.weight [p*p*out_channels, D] */
   const float* final_b;
   const void* final_w16;   /* 16-bit copy of final_w (tensor-core head) or NULL */
+  /* FP8 sampling path (opt-in; NULL = the 16-bit GEMM), the contract of B200LatteWeights.qkv_w8 ...: e4m3 copies of the four
+   * stacks fed by LayerNorm + modulate, stacked over layers like their 16-bit copies, with one fp32 scale per output channel,
+   * as b200_quantize_rows_e4m3 makes them.  When a stack's e4m3 copy is set, its LayerNorm + modulate writes e4m3 with one
+   * scale per token and the GEMM multiplies e4m3 on the tensor cores; its 16-bit copy is not read and may be NULL.  Every
+   * other GEMM (out-projections, attn2's query, the caption projection and K/V, fc2, the head) stays 16-bit. */
+  const void* s_qkv_w8;    /* transformer_blocks.l.attn1.to_q|to_k|to_v.weight [l][3D, D] e4m3 */
+  const float* s_qkv_ws;   /*                                                 [l][3D] scales */
+  const void* s_fc1_w8;    /* transformer_blocks.l.ff.net.0.proj.weight       [l][4D, D] e4m3 */
+  const float* s_fc1_ws;   /*                                                 [l][4D] scales */
+  const void* t_qkv_w8;    /* temporal_transformer_blocks.l.attn1.to_q|to_k|to_v.weight [l][3D, D] e4m3 */
+  const float* t_qkv_ws;   /*                                                 [l][3D] scales */
+  const void* t_fc1_w8;    /* temporal_transformer_blocks.l.ff.net.0.proj.weight [l][4D, D] e4m3 */
+  const float* t_fc1_ws;   /*                                                 [l][4D] scales */
 } B200T2VWeights;
 
 B200_API size_t b200_t2v_workspace_bytes(const B200T2VShape* shape, int batch, int text_len);

@@ -10,7 +10,7 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buffer
 OK = 0
 FP16, BF16 = 0, 1
@@ -47,7 +47,7 @@ T2V_WEIGHT_FIELDS = (
     "s_qkv_w16", "s_qkv_b", "s_out_w16", "s_out_b", "c_q_w16", "c_q_b", "c_kv_w16", "c_kv_b", "c_out_w16", "c_out_b",
     "s_fc1_w16", "s_fc1_b", "s_fc2_w16", "s_fc2_b",
     "t_qkv_w16", "t_qkv_b", "t_out_w16", "t_out_b", "t_fc1_w16", "t_fc1_b", "t_fc2_w16", "t_fc2_b", "final_w", "final_b",
-    "final_w16")
+    "final_w16", "s_qkv_w8", "s_qkv_ws", "s_fc1_w8", "s_fc1_ws", "t_qkv_w8", "t_qkv_ws", "t_fc1_w8", "t_fc1_ws")
 
 
 class T2VWeights(C.Structure):

@@ -121,6 +121,31 @@ size_t conditioning_scratch_bytes(const B200LatteShape* s, int n) {
   return align_up(static_cast<size_t>(n) * 256 * 4, 1024) + 2 * align_up(static_cast<size_t>(n) * s->hidden * 4, 1024);
 }
 
+// ---- LayerNorm + modulate of the residual stream x, then the GEMM it feeds: layer i's QKV (B200_EPI_BIAS) or fc1
+// (B200_EPI_BIAS_GELU) of a weight stack [layers][N, D] -> out16 [T, N].  Latte's blocks and both LatteT2V blocks make this
+// one choice: with an e4m3 copy of the stack (w8, w_scale [layers][N]) the LN output is quantized per token and the GEMM
+// runs on e4m3 tensor cores; else the 16-bit LN output and weight.  The e4m3 operand and its row scales (T*D + 4T bytes)
+// live in h (T*D*2 bytes), which the GEMM consumes before anything else writes h.
+int ln_modulate_linear(const float* x, const float* shift, const float* scale, long long mod_bs, int rows_per_batch,
+                       uint16_t* h, int T, int D, const void* w16, const void* w8, const float* w_scale, const float* bias,
+                       int i, int N, int epilogue, int bf16, void* out16, cudaStream_t stream) {
+  const size_t w_off = static_cast<size_t>(i) * N * D, n_off = static_cast<size_t>(i) * N;
+  if (w8) {
+    uint8_t* h8 = reinterpret_cast<uint8_t*>(h);
+    float* h8_scale = reinterpret_cast<float*>(h8 + static_cast<size_t>(T) * D);
+    B200_PROF(PROF_LN, launch_ln_modulate_e4m3(x, shift, scale, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
+    B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w8) + w_off, w_scale + n_off, bias + n_off,
+                                            T, N, D, bf16, epilogue, out16, stream));
+    return B200_OK;
+  }
+  B200_PROF(PROF_LN, launch_ln_modulate(x, shift, scale, mod_bs, rows_per_batch, h, T, D, bf16, stream));
+  GemmArgs g{};
+  g.A = h; g.W = static_cast<const uint16_t*>(w16) + w_off; g.bias = bias + n_off;
+  g.M = T; g.N = N; g.K = D; g.bf16 = bf16; g.epilogue = epilogue; g.out16 = out16; g.w_const = 1;
+  B200_PROF(PROF_GEMM, launch_gemm(g, stream));
+  return B200_OK;
+}
+
 // premod != NULL: the caller already holds this batch's conditioning rows (b200_latte_conditioning, e.g. for a whole
 // sampling trajectory at once -- SURVEY.md 8f rank 2); t is then unused and the adaLN weights are not read.
 int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, const int64_t* t, const int64_t* y,
@@ -150,10 +175,6 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   B200_REQUIRE((!w->qkv_w8 || w->qkv_ws) && (!w->fc1_w8 || w->fc1_ws), B200_ERR_SHAPE, "e4m3 weights need their scales");
   B200_REQUIRE((w->qkv_w8 || w->qkv_w16) && (w->fc1_w8 || w->fc1_w16), B200_ERR_SHAPE,
                "qkv and fc1 need a 16-bit or an e4m3 weight copy");
-  // FP8 path: the e4m3 operand of QKV / fc1 and its row scales (T*D + 4T bytes) live in ws.h (T*D*2 bytes), which the GEMM
-  // consumes before attention or the next LayerNorm overwrites it
-  uint8_t* h8 = reinterpret_cast<uint8_t*>(ws.h);
-  float* h8_scale = reinterpret_cast<float*>(h8 + static_cast<size_t>(T) * D);
 
   // stream-K ordering flags: zero at the start of the step (every stream-K GEMM leaves them zero again; this memset only
   // makes the step independent of whatever the workspace held before -- a fresh allocation, an aborted run)
@@ -171,18 +192,8 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
     const uint16_t* proj_w = static_cast<const uint16_t*>(w->proj_w16) + static_cast<size_t>(i) * D * D;
     const uint16_t* fc2_w = static_cast<const uint16_t*>(w->fc2_w16) + static_cast<size_t>(i) * D * HID;
 
-    if (w->qkv_w8) {
-      B200_PROF(PROF_LN, launch_ln_modulate_e4m3(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
-      B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w->qkv_w8) + static_cast<size_t>(i) * 3 * D * D,
-                                              w->qkv_ws + static_cast<size_t>(i) * 3 * D, w->qkv_b + static_cast<size_t>(i) * 3 * D,
-                                              T, 3 * D, D, bf16, B200_EPI_BIAS, ws.qkv, stream));
-    } else {
-      B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-      GemmArgs ga{};
-      ga.A = ws.h; ga.W = static_cast<const uint16_t*>(w->qkv_w16) + static_cast<size_t>(i) * 3 * D * D; ga.bias = w->qkv_b + static_cast<size_t>(i) * 3 * D;
-      ga.M = T; ga.N = 3 * D; ga.K = D; ga.bf16 = bf16; ga.epilogue = B200_EPI_BIAS; ga.out16 = ws.qkv; ga.w_const = 1;
-      B200_PROF(PROF_GEMM, launch_gemm(ga, stream));
-    }
+    B200_TRY(ln_modulate_linear(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->qkv_w16, w->qkv_w8, w->qkv_ws,
+                                w->qkv_b, i, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
 
     AttnArgs aa{};
     aa.qkv = ws.qkv; aa.out = ws.h; aa.batch = batch; aa.frames = F; aa.tokens = N; aa.heads = H; aa.head_dim = hd;
@@ -195,18 +206,8 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
     gp.gate = m + 2 * D; gp.gate_batch_stride = mod_bs; gp.rows_per_batch = rows_per_batch; gp.sk_flags = ws.sk_flags;
     B200_PROF(PROF_GEMM, launch_gemm(gp, stream));
 
-    if (w->fc1_w8) {
-      B200_PROF(PROF_LN, launch_ln_modulate_e4m3(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
-      B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w->fc1_w8) + static_cast<size_t>(i) * HID * D,
-                                              w->fc1_ws + static_cast<size_t>(i) * HID, w->fc1_b + static_cast<size_t>(i) * HID,
-                                              T, HID, D, bf16, B200_EPI_BIAS_GELU, ws.g, stream));
-    } else {
-      B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-      GemmArgs g1{};
-      g1.A = ws.h; g1.W = static_cast<const uint16_t*>(w->fc1_w16) + static_cast<size_t>(i) * HID * D; g1.bias = w->fc1_b + static_cast<size_t>(i) * HID;
-      g1.M = T; g1.N = HID; g1.K = D; g1.bf16 = bf16; g1.epilogue = B200_EPI_BIAS_GELU; g1.out16 = ws.g; g1.w_const = 1;
-      B200_PROF(PROF_GEMM, launch_gemm(g1, stream));
-    }
+    B200_TRY(ln_modulate_linear(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->fc1_w16, w->fc1_w8, w->fc1_ws,
+                                w->fc1_b, i, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
 
     GemmArgs g2{};
     g2.A = ws.g; g2.W = fc2_w; g2.bias = w->fc2_b + static_cast<size_t>(i) * D;
@@ -303,6 +304,12 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   const int rows_per_batch = F * N;
   const int bf16 = s->dtype == B200_BF16;
   const long long mod_bs = static_cast<long long>(L) * 2 * 6 * D + 2 * D;
+  B200_REQUIRE((!w->s_qkv_w8 || w->s_qkv_ws) && (!w->s_fc1_w8 || w->s_fc1_ws) && (!w->t_qkv_w8 || w->t_qkv_ws) &&
+                   (!w->t_fc1_w8 || w->t_fc1_ws),
+               B200_ERR_SHAPE, "t2v: e4m3 weights need their scales");
+  B200_REQUIRE((w->s_qkv_w8 || w->s_qkv_w16) && (w->s_fc1_w8 || w->s_fc1_w16) && (w->t_qkv_w8 || w->t_qkv_w16) &&
+                   (w->t_fc1_w8 || w->t_fc1_w16),
+               B200_ERR_SHAPE, "t2v: qkv and fc1 need a 16-bit or an e4m3 weight copy");
 
   B200_CHECK_CUDA(cudaMemsetAsync(ws.sk_flags, 0, static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8, stream));
   // ---- conditioning (latte_t2v.py:782-784): emb = TimestepEmbedding(sincos(t)); ts = Linear(SiLU(emb)); tables + ts
@@ -352,9 +359,8 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   for (int l = 0; l < L; ++l) {
     // ------------------------------------------------ spatial block (diffusers BasicTransformerBlock; latte_t2v.py:862-870)
     const float* m = ws.mod + static_cast<size_t>(2 * l) * 6 * D;
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->s_qkv_w16) + l * 3 * DD, w->s_qkv_b + static_cast<size_t>(l) * 3 * D,
-                                  T, 3 * D, D, B200_EPI_BIAS, ws.qkv));
+    B200_TRY(ln_modulate_linear(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->s_qkv_w16, w->s_qkv_w8,
+                                w->s_qkv_ws, w->s_qkv_b, l, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
     AttnArgs aa{};
     aa.qkv = ws.qkv; aa.out = ws.h; aa.batch = batch; aa.frames = F; aa.tokens = N; aa.heads = H; aa.head_dim = hd; aa.bf16 = bf16;
     aa.temporal = 0;
@@ -372,9 +378,8 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
     B200_PROF(PROF_ATTN, launch_cross_attention(ca, stream));
     B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->c_out_w16) + l * DD, w->c_out_b + static_cast<size_t>(l) * D, D,
                                       ws.ones, 0, nullptr));
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->s_fc1_w16) + static_cast<size_t>(l) * HID * D,
-                                  w->s_fc1_b + static_cast<size_t>(l) * HID, T, HID, D, B200_EPI_BIAS_GELU, ws.g));
+    B200_TRY(ln_modulate_linear(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->s_fc1_w16, w->s_fc1_w8,
+                                w->s_fc1_ws, w->s_fc1_b, l, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
     // + temp_pos_embed before the first temporal block (latte_t2v.py:894-895), folded into this epilogue
     B200_PROF(PROF_GEMM, linear_resid(ws.g, static_cast<const uint16_t*>(w->s_fc2_w16) + static_cast<size_t>(l) * D * HID,
                                       w->s_fc2_b + static_cast<size_t>(l) * D, HID, m + 5 * D, mod_bs,
@@ -382,16 +387,14 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
     if (!enable_temporal) continue;
     // ------------------------------------------------ temporal block (BasicTransformerBlock_, latte_t2v.py:897-905)
     const float* mt = ws.mod + static_cast<size_t>(2 * l + 1) * 6 * D;
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, mt + 0 * D, mt + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->t_qkv_w16) + l * 3 * DD, w->t_qkv_b + static_cast<size_t>(l) * 3 * D,
-                                  T, 3 * D, D, B200_EPI_BIAS, ws.qkv));
+    B200_TRY(ln_modulate_linear(ws.x, mt + 0 * D, mt + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->t_qkv_w16, w->t_qkv_w8,
+                                w->t_qkv_ws, w->t_qkv_b, l, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
     aa.temporal = 1;
     B200_PROF(PROF_ATTN, launch_attention(aa, stream));
     B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->t_out_w16) + l * DD, w->t_out_b + static_cast<size_t>(l) * D, D,
                                       mt + 2 * D, mod_bs, nullptr));
-    B200_PROF(PROF_LN, launch_ln_modulate(ws.x, mt + 3 * D, mt + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->t_fc1_w16) + static_cast<size_t>(l) * HID * D,
-                                  w->t_fc1_b + static_cast<size_t>(l) * HID, T, HID, D, B200_EPI_BIAS_GELU, ws.g));
+    B200_TRY(ln_modulate_linear(ws.x, mt + 3 * D, mt + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->t_fc1_w16, w->t_fc1_w8,
+                                w->t_fc1_ws, w->t_fc1_b, l, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
     B200_PROF(PROF_GEMM, linear_resid(ws.g, static_cast<const uint16_t*>(w->t_fc2_w16) + static_cast<size_t>(l) * D * HID,
                                       w->t_fc2_b + static_cast<size_t>(l) * D, HID, mt + 5 * D, mod_bs, nullptr));
   }
