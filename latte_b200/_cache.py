@@ -7,6 +7,8 @@ copy must not alias another instance's buffers, so `copy.deepcopy(model)` (the E
 """
 from __future__ import annotations
 
+import torch
+
 
 class DeviceCacheMixin:
     _CACHE_ATTRS = {"_packed": None, "_packed_key": None, "_workspace": None, "_trajectory": None, "_graphs": None,
@@ -18,3 +20,11 @@ class DeviceCacheMixin:
             if k in state:
                 state[k] = empty
         return state
+
+    def _aligned_workspace(self, need: int, device) -> int:
+        """Device address of `need` bytes of scratch on a 1024-byte boundary, inside `_workspace` (reallocated when it is too
+        small or on another device)."""
+        ws = self._workspace
+        if ws is None or ws.numel() < need + 1024 or ws.device != device:
+            ws = self._workspace = torch.empty(need + 1024, dtype=torch.uint8, device=device)
+        return (ws.data_ptr() + 1023) // 1024 * 1024

@@ -41,6 +41,181 @@ struct ProfScope {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// ---- workspace arena: consecutive buffers from `base`, each starting on a 1024-byte boundary; base == NULL only sizes them
+struct Arena {
+  uint8_t* base;
+  size_t off = 0;
+  template <class T>
+  T* take(size_t bytes) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += align_up(bytes, 1024);
+    return p;
+  }
+};
+
+// ---- shape rules Latte and LatteT2V share: head_dim, the GEMM K tile, the patch size, the operand type and the head width.
+// `who` prefixes the message ("" for Latte, "t2v: " for LatteT2V).
+template <class Shape>
+int block_shape_ok(const char* who, const Shape* s, int batch) {
+  B200_REQUIRE(s != nullptr && batch > 0, B200_ERR_SHAPE, "%sshape is NULL or batch %d is not positive", who, batch);
+  B200_REQUIRE(s->heads > 0 && s->hidden % s->heads == 0, B200_ERR_SHAPE, "%shidden %d not divisible by heads %d", who, s->hidden,
+               s->heads);
+  const int hd = s->hidden / s->heads;
+  B200_REQUIRE(hd == 64 || hd == 72 || hd == 80, B200_ERR_UNSUPPORTED, "%shead_dim %d unsupported", who, hd);
+  B200_REQUIRE(s->hidden % 64 == 0 && s->mlp_hidden % 64 == 0, B200_ERR_UNSUPPORTED,
+               "%shidden %d and mlp_hidden %d must be multiples of 64 (GEMM K tile)", who, s->hidden, s->mlp_hidden);
+  B200_REQUIRE(s->patch == 2, B200_ERR_UNSUPPORTED, "%spatch size %d not built (only 2)", who, s->patch);
+  B200_REQUIRE(s->input_size % s->patch == 0, B200_ERR_SHAPE, "%sinput_size %d not divisible by patch", who, s->input_size);
+  B200_REQUIRE(s->dtype == B200_FP16 || s->dtype == B200_BF16, B200_ERR_DTYPE, "%sdtype %d unknown", who, s->dtype);
+  B200_REQUIRE(s->out_channels * s->patch * s->patch <= 32, B200_ERR_UNSUPPORTED, "%sp*p*out_channels > 32", who);
+  return B200_OK;
+}
+
+// ---- the forwards' two GEMM shapes.  linear16: out16[M, N] = epilogue(A[M, K] . W[N, K]^T + bias) in 16 bits
+// (B200_EPI_BIAS, B200_EPI_BIAS_GELU, or B200_EPI_BIAS_MUL16, which multiplies by mul16 [M, N]).
+int linear16(const void* A, const void* W, const float* bias, int M, int N, int K, int bf16, int epilogue, void* out16,
+             cudaStream_t stream, const void* mul16 = nullptr) {
+  GemmArgs g{};
+  g.A = A; g.W = W; g.bias = bias; g.M = M; g.N = N; g.K = K; g.bf16 = bf16; g.epilogue = epilogue; g.out16 = out16; g.add16 = mul16;
+  return launch_gemm(g, stream);
+}
+
+// linear_resid: the gated residual into an fp32 stream, resid[M, N] += gate[(row / rows_per_batch) * gate_bs + col] *
+// (A . W^T + bias), plus row_add[((row / row_add_div) % row_add_period) * N + col] when row_add is set.
+int linear_resid(const void* A, const void* W, const float* bias, int M, int N, int K, int bf16, float* resid,
+                 const float* gate, long long gate_bs, int rows_per_batch, unsigned long long* sk_flags, cudaStream_t stream,
+                 const float* row_add = nullptr, int row_add_div = 0, int row_add_period = 0) {
+  GemmArgs g{};
+  g.A = A; g.W = W; g.bias = bias; g.M = M; g.N = N; g.K = K; g.bf16 = bf16; g.epilogue = B200_EPI_GATE_RESIDUAL;
+  g.resid = resid; g.gate = gate; g.gate_batch_stride = gate_bs; g.rows_per_batch = rows_per_batch; g.sk_flags = sk_flags;
+  g.row_add = row_add; g.row_add_div = row_add_div; g.row_add_period = row_add_period;
+  return launch_gemm(g, stream);
+}
+
+// ---- timestep embedding of n rows, both models: c = Linear(D, D)(SiLU(Linear(256, D)(tfreq = sincos(t)))) (+ y_table[y])
+template <class Weights>
+int timestep_embedding(const Weights* w, const int64_t* t, const float* y_table, const int64_t* y, int num_embed, int n,
+                       int D, float* tfreq, float* th, float* c, cudaStream_t stream) {
+  B200_PROF(PROF_OTHER, launch_timestep_freq(reinterpret_cast<const long long*>(t), tfreq, n, stream));
+  B200_PROF(PROF_OTHER, launch_gemv(w->t_w0, 32, 0, w->t_b0, tfreq, th, n, D, 256, 0, 1, nullptr, nullptr, 0, stream));
+  B200_PROF(PROF_OTHER, launch_gemv(w->t_w2, 32, 0, w->t_b2, th, c, n, D, D, 0, 0, y_table, reinterpret_cast<const long long*>(y),
+                                    num_embed, stream));
+  return B200_OK;
+}
+
+// ====================================================================================================== transformer block
+// The launch sequence of one Latte block, and of each LatteT2V spatial and temporal block:
+//   attention half: LN + modulate -> QKV -> self-attention -> x += gate * out-projection
+//   mlp half:       LN + modulate -> fc1 (+GELU) -> x += gate * fc2 (+ row_add)
+// A LatteT2V spatial block runs its cross-attention step between the two halves.
+
+// The forward's fp32 residual stream x [T = batch*F*N, D], its scratch h [T, D] (LN + modulate output, then attention output),
+// qkv [T, 3D] and g [T, mlp_hidden], and its geometry; mod_bs is the per-sample stride of the modulation rows.
+struct Step {
+  float* x; uint16_t* h; uint16_t* qkv; uint16_t* g; unsigned long long* sk_flags;
+  int batch, F, N, heads, D, mlp_hidden;
+  long long mod_bs;
+  int bf16;
+  cudaStream_t stream;
+  int T() const { return batch * F * N; }
+};
+
+// One block's operands, offset to its layer (`layer`): weights [N, K] 16-bit or e4m3, per-channel e4m3 scales and fp32
+// biases [N].  A 16-bit QKV or fc1 copy may be NULL beside an e4m3 one.
+struct BlockWeights {
+  const void* qkv_w16; const void* qkv_w8; const float* qkv_ws; const float* qkv_b;
+  const void* out_w16; const float* out_b;
+  const void* fc1_w16; const void* fc1_w8; const float* fc1_ws; const float* fc1_b;
+  const void* fc2_w16; const float* fc2_b;
+};
+
+// a block's QKV and fc1 stacks each need a 16-bit copy or an e4m3 one with its per-channel scales (`who`: message prefix)
+int e4m3_stacks_ok(const char* who, const BlockWeights& b) {
+  B200_REQUIRE(b.qkv_w8 ? b.qkv_ws != nullptr : b.qkv_w16 != nullptr, B200_ERR_SHAPE,
+               "%sqkv needs a 16-bit weight copy or an e4m3 one with its scales", who);
+  B200_REQUIRE(b.fc1_w8 ? b.fc1_ws != nullptr : b.fc1_w16 != nullptr, B200_ERR_SHAPE,
+               "%sfc1 needs a 16-bit weight copy or an e4m3 one with its scales", who);
+  return B200_OK;
+}
+
+// layer i of the stacks [layers][...] that `stack` points at
+BlockWeights layer(const BlockWeights& stack, int i, size_t D, size_t HID) {
+  auto w16 = [i](const void* p, size_t n) -> const void* { return p ? static_cast<const uint16_t*>(p) + i * n : nullptr; };
+  auto w8 = [i](const void* p, size_t n) -> const void* { return p ? static_cast<const uint8_t*>(p) + i * n : nullptr; };
+  auto f32 = [i](const float* p, size_t n) -> const float* { return p ? p + i * n : nullptr; };
+  return {w16(stack.qkv_w16, 3 * D * D), w8(stack.qkv_w8, 3 * D * D), f32(stack.qkv_ws, 3 * D), f32(stack.qkv_b, 3 * D),
+          w16(stack.out_w16, D * D), f32(stack.out_b, D),
+          w16(stack.fc1_w16, HID * D), w8(stack.fc1_w8, HID * D), f32(stack.fc1_ws, HID), f32(stack.fc1_b, HID),
+          w16(stack.fc2_w16, D * HID), f32(stack.fc2_b, D)};
+}
+
+// LayerNorm + modulate of the residual stream, then the GEMM it feeds (QKV with B200_EPI_BIAS, fc1 with B200_EPI_BIAS_GELU)
+// -> out16 [T, N].  With an e4m3 weight copy (w8, w_scale [N]) the LN output is quantized per token and the GEMM runs on
+// e4m3 tensor cores; else the 16-bit LN output and weight.  The e4m3 operand and its row scales (T*D + 4T bytes) live in h
+// (T*D*2 bytes), which the GEMM consumes before anything else writes h.
+int ln_modulate_linear(const Step& s, const float* shift, const float* scale, const void* w16, const void* w8,
+                       const float* w_scale, const float* bias, int N, int epilogue, void* out16) {
+  cudaStream_t stream = s.stream;
+  const int T = s.T();
+  if (w8) {
+    uint8_t* h8 = reinterpret_cast<uint8_t*>(s.h);
+    float* h8_scale = reinterpret_cast<float*>(h8 + static_cast<size_t>(T) * s.D);
+    B200_PROF(PROF_LN, launch_ln_modulate_e4m3(s.x, shift, scale, s.mod_bs, s.F * s.N, h8, h8_scale, T, s.D, stream));
+    B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, w8, w_scale, bias, T, N, s.D, s.bf16, epilogue, out16, stream));
+    return B200_OK;
+  }
+  B200_PROF(PROF_LN, launch_ln_modulate(s.x, shift, scale, s.mod_bs, s.F * s.N, s.h, T, s.D, s.bf16, stream));
+  B200_PROF(PROF_GEMM, linear16(s.h, w16, bias, T, N, s.D, s.bf16, epilogue, out16, stream));
+  return B200_OK;
+}
+
+// m: the block's modulation rows [shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp], each [D]
+int attention_half(const Step& s, const BlockWeights& b, const float* m, int temporal) {
+  const int D = s.D;
+  cudaStream_t stream = s.stream;
+  B200_TRY(ln_modulate_linear(s, m + 0 * D, m + 1 * D, b.qkv_w16, b.qkv_w8, b.qkv_ws, b.qkv_b, 3 * D, B200_EPI_BIAS, s.qkv));
+  AttnArgs aa{};
+  aa.qkv = s.qkv; aa.out = s.h; aa.batch = s.batch; aa.frames = s.F; aa.tokens = s.N; aa.heads = s.heads; aa.head_dim = D / s.heads;
+  aa.bf16 = s.bf16; aa.temporal = temporal;
+  B200_PROF(PROF_ATTN, launch_attention(aa, stream));
+  B200_PROF(PROF_GEMM, linear_resid(s.h, b.out_w16, b.out_b, s.T(), D, D, s.bf16, s.x, m + 2 * D, s.mod_bs, s.F * s.N, s.sk_flags,
+                                    stream));
+  return B200_OK;
+}
+
+// row_add: NULL, or a [frames, D] table added to every token of each frame in fc2's epilogue
+int mlp_half(const Step& s, const BlockWeights& b, const float* m, const float* row_add) {
+  const int D = s.D;
+  cudaStream_t stream = s.stream;
+  B200_TRY(ln_modulate_linear(s, m + 3 * D, m + 4 * D, b.fc1_w16, b.fc1_w8, b.fc1_ws, b.fc1_b, s.mlp_hidden, B200_EPI_BIAS_GELU,
+                              s.g));
+  B200_PROF(PROF_GEMM, linear_resid(s.g, b.fc2_w16, b.fc2_b, s.T(), D, s.mlp_hidden, s.bf16, s.x, m + 5 * D, s.mod_bs, s.F * s.N,
+                                    s.sk_flags, stream, row_add, row_add ? s.N : 0, row_add ? s.F : 0));
+  return B200_OK;
+}
+
+// ---- output head (latte.py:197-201,297-310,374-376): LayerNorm + modulate -> Linear(D, p*p*C_out) -> unpatchify.
+// With a 16-bit weight copy and p*p*C_out == 32 the Linear runs on the tensor cores: the GEMM's gated-residual epilogue on a
+// zeroed fp32 buffer with gate = 1 IS "fp32 out = acc + bias".  Otherwise the fp32 CUDA-core kernel.
+int output_head(const float* x, uint16_t* h, float* head, const float* shift, const float* scale, long long mod_bs,
+                const float* w32, const void* w16, const float* bias, float* out, int batch, int F, int grid, int patch,
+                int out_ch, int D, int bf16, int channels_first, unsigned long long* sk_flags, cudaStream_t stream) {
+  const int n_out = patch * patch * out_ch;
+  const int T = batch * F * grid * grid;
+  if (w16 == nullptr || n_out != 32) {
+    B200_PROF(PROF_OTHER, launch_final_layer(x, shift, scale, mod_bs, w32, bias, out, batch, F, grid, patch, out_ch, D, channels_first, stream));
+    return B200_OK;
+  }
+  float* ones = head + static_cast<size_t>(T) * 32;
+  B200_CHECK_CUDA(cudaMemsetAsync(head, 0, static_cast<size_t>(T) * 32 * 4, stream));
+  B200_PROF(PROF_OTHER, launch_fill(ones, 1.0f, 32, stream));
+  B200_PROF(PROF_LN, launch_ln_modulate(x, shift, scale, mod_bs, F * grid * grid, h, T, D, bf16, stream));
+  B200_PROF(PROF_GEMM, linear_resid(h, w16, bias, T, n_out, D, bf16, head, ones, 0, T, sk_flags, stream));
+  B200_PROF(PROF_OTHER, launch_unpatchify(head, out, batch, F, grid, patch, out_ch, channels_first, stream));
+  return B200_OK;
+}
+
+// ====================================================================================================== Latte
 struct Workspace {
   float* x;          // [T, D]   fp32 residual stream, rows (b, f, n)
   uint16_t* h;       // [T, D]   16-bit: LN+modulate output, then attention output
@@ -52,97 +227,45 @@ struct Workspace {
   float* mod;        // [B, depth*6D + 2D]
   unsigned long long* sk_flags;   // [B200_GEMM_SK_FLAGS] stream-K ordering flags (zeroed at the start of every forward)
   float* head;       // [T, 32]  fp32 output of the head GEMM (zeroed, then reduce-added into), followed by 32 ones (its "gate")
-  size_t bytes;
 };
 
-// ---- output head (latte.py:197-201,297-310,374-376): LayerNorm + modulate -> Linear(D, p*p*C_out) -> unpatchify.
-// With a 16-bit weight copy and p*p*C_out a multiple of 32 the Linear runs on the tensor cores: the GEMM's gated-residual
-// epilogue on a zeroed fp32 buffer with gate = 1 IS "fp32 out = acc + bias".  Otherwise the fp32 CUDA-core kernel.
-int output_head(const float* x, uint16_t* h, float* head, const float* shift, const float* scale, long long mod_bs,
-                const float* w32, const void* w16, const float* bias, float* out, int batch, int F, int grid, int patch,
-                int out_ch, int D, int bf16, int channels_first, unsigned long long* sk_flags, cudaStream_t stream);
-
 int shape_ok(const B200LatteShape* s, int batch) {
-  B200_REQUIRE(s != nullptr, B200_ERR_SHAPE, "shape is NULL");
-  B200_REQUIRE(batch > 0, B200_ERR_SHAPE, "batch %d must be positive", batch);
+  B200_TRY(block_shape_ok("", s, batch));
   B200_REQUIRE(s->depth > 0 && s->depth % 2 == 0, B200_ERR_SHAPE, "depth %d must be even (spatial/temporal pairs)", s->depth);
-  B200_REQUIRE(s->heads > 0 && s->hidden % s->heads == 0, B200_ERR_SHAPE, "hidden %d not divisible by heads %d", s->hidden, s->heads);
-  const int hd = s->hidden / s->heads;
-  B200_REQUIRE(hd == 64 || hd == 72 || hd == 80, B200_ERR_UNSUPPORTED, "head_dim %d unsupported", hd);
-  B200_REQUIRE(s->hidden % 64 == 0 && s->mlp_hidden % 64 == 0, B200_ERR_UNSUPPORTED,
-               "hidden %d and mlp_hidden %d must be multiples of 64 (GEMM K tile)", s->hidden, s->mlp_hidden);
-  B200_REQUIRE(s->patch == 2, B200_ERR_UNSUPPORTED, "patch size %d not built (only 2)", s->patch);
-  B200_REQUIRE(s->input_size % s->patch == 0, B200_ERR_SHAPE, "input_size %d not divisible by patch", s->input_size);
-  B200_REQUIRE(s->dtype == B200_FP16 || s->dtype == B200_BF16, B200_ERR_DTYPE, "dtype %d unknown", s->dtype);
-  B200_REQUIRE(s->out_channels * s->patch * s->patch <= 32, B200_ERR_UNSUPPORTED, "p*p*out_channels > 32");
   return B200_OK;
 }
 
-void carve(const B200LatteShape* s, int batch, void* base, Workspace* ws) {
+// carves `base` (NULL: sizes only) and returns the bytes it needs
+size_t carve(const B200LatteShape* s, int batch, void* base, Workspace* ws) {
   const size_t grid = s->input_size / s->patch;
-  const size_t T = static_cast<size_t>(batch) * s->frames * grid * grid;
-  const size_t D = s->hidden;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    void* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
-    off += align_up(bytes, 1024);
-    return p;
-  };
-  ws->x = static_cast<float*>(take(T * D * 4));
-  ws->h = static_cast<uint16_t*>(take(T * D * 2));
-  ws->qkv = static_cast<uint16_t*>(take(T * 3 * D * 2));
-  ws->g = static_cast<uint16_t*>(take(T * static_cast<size_t>(s->mlp_hidden) * 2));
-  ws->tfreq = static_cast<float*>(take(static_cast<size_t>(batch) * 256 * 4));
-  ws->th = static_cast<float*>(take(static_cast<size_t>(batch) * D * 4));
-  ws->c = static_cast<float*>(take(static_cast<size_t>(batch) * D * 4));
-  ws->mod = static_cast<float*>(take(static_cast<size_t>(batch) * (static_cast<size_t>(s->depth) * 6 * D + 2 * D) * 4));
-  ws->sk_flags = static_cast<unsigned long long*>(take(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8));
-  ws->head = static_cast<float*>(take((T + 1) * 32 * 4));
-  ws->bytes = off;
+  const size_t B = batch, T = B * s->frames * grid * grid, D = s->hidden;
+  Arena a{static_cast<uint8_t*>(base)};
+  ws->x = a.take<float>(T * D * 4);
+  ws->h = a.take<uint16_t>(T * D * 2);
+  ws->qkv = a.take<uint16_t>(T * 3 * D * 2);
+  ws->g = a.take<uint16_t>(T * s->mlp_hidden * 2);
+  ws->tfreq = a.take<float>(B * 256 * 4);
+  ws->th = a.take<float>(B * D * 4);
+  ws->c = a.take<float>(B * D * 4);
+  ws->mod = a.take<float>(B * (s->depth * 6 * D + 2 * D) * 4);
+  ws->sk_flags = a.take<unsigned long long>(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8);
+  ws->head = a.take<float>((T + 1) * 32 * 4);
+  return a.off;
+}
+
+// b200_latte_conditioning's scratch: tfreq [n, 256], th [n, D], c [n, D]
+size_t conditioning_scratch_bytes(const B200LatteShape* s, int n) {
+  return align_up(static_cast<size_t>(n) * 256 * 4, 1024) + 2 * align_up(static_cast<size_t>(n) * s->hidden * 4, 1024);
 }
 
 // ---- conditioning, once per SAMPLE (latte.py:332-339): c = t_embedder(t) (+ y_embedder(y)); mod = adaLN(SiLU(c)) for all
 // blocks and the final layer.  `n` rows; scratch tfreq [n,256], th [n,D], c [n,D]; mod [n, depth*6D + 2D].
 int conditioning(const B200LatteShape* s, const B200LatteWeights* w, const int64_t* t, const int64_t* y, int n, float* tfreq,
                  float* th, float* c, float* mod, cudaStream_t stream) {
-  const int D = s->hidden;
-  const int bf16 = s->dtype == B200_BF16;
-  const long long mod_bs = static_cast<long long>(s->depth) * 6 * D + 2 * D;
-  B200_PROF(PROF_OTHER, launch_timestep_freq(reinterpret_cast<const long long*>(t), tfreq, n, stream));
-  B200_PROF(PROF_OTHER, launch_gemv(w->t_w0, 32, 0, w->t_b0, tfreq, th, n, D, 256, 0, 1, nullptr, nullptr, 0, stream));
-  B200_PROF(PROF_OTHER, launch_gemv(w->t_w2, 32, 0, w->t_b2, th, c, n, D, D, 0, 0, s->num_embed > 0 ? w->y_table : nullptr,
-                       reinterpret_cast<const long long*>(y), s->num_embed, stream));
-  B200_PROF(PROF_OTHER, launch_gemv(w->ada_w16, 16, bf16, w->ada_b, c, mod, n, static_cast<int>(mod_bs), D, 1, 0, nullptr,
-                       nullptr, 0, stream));
-  return B200_OK;
-}
-
-size_t conditioning_scratch_bytes(const B200LatteShape* s, int n) {
-  return align_up(static_cast<size_t>(n) * 256 * 4, 1024) + 2 * align_up(static_cast<size_t>(n) * s->hidden * 4, 1024);
-}
-
-// ---- LayerNorm + modulate of the residual stream x, then the GEMM it feeds: layer i's QKV (B200_EPI_BIAS) or fc1
-// (B200_EPI_BIAS_GELU) of a weight stack [layers][N, D] -> out16 [T, N].  Latte's blocks and both LatteT2V blocks make this
-// one choice: with an e4m3 copy of the stack (w8, w_scale [layers][N]) the LN output is quantized per token and the GEMM
-// runs on e4m3 tensor cores; else the 16-bit LN output and weight.  The e4m3 operand and its row scales (T*D + 4T bytes)
-// live in h (T*D*2 bytes), which the GEMM consumes before anything else writes h.
-int ln_modulate_linear(const float* x, const float* shift, const float* scale, long long mod_bs, int rows_per_batch,
-                       uint16_t* h, int T, int D, const void* w16, const void* w8, const float* w_scale, const float* bias,
-                       int i, int N, int epilogue, int bf16, void* out16, cudaStream_t stream) {
-  const size_t w_off = static_cast<size_t>(i) * N * D, n_off = static_cast<size_t>(i) * N;
-  if (w8) {
-    uint8_t* h8 = reinterpret_cast<uint8_t*>(h);
-    float* h8_scale = reinterpret_cast<float*>(h8 + static_cast<size_t>(T) * D);
-    B200_PROF(PROF_LN, launch_ln_modulate_e4m3(x, shift, scale, mod_bs, rows_per_batch, h8, h8_scale, T, D, stream));
-    B200_PROF(PROF_GEMM, launch_linear_e4m3(h8, h8_scale, static_cast<const uint8_t*>(w8) + w_off, w_scale + n_off, bias + n_off,
-                                            T, N, D, bf16, epilogue, out16, stream));
-    return B200_OK;
-  }
-  B200_PROF(PROF_LN, launch_ln_modulate(x, shift, scale, mod_bs, rows_per_batch, h, T, D, bf16, stream));
-  GemmArgs g{};
-  g.A = h; g.W = static_cast<const uint16_t*>(w16) + w_off; g.bias = bias + n_off;
-  g.M = T; g.N = N; g.K = D; g.bf16 = bf16; g.epilogue = epilogue; g.out16 = out16; g.w_const = 1;
-  B200_PROF(PROF_GEMM, launch_gemm(g, stream));
+  const int D = s->hidden, mod_rows = s->depth * 6 * D + 2 * D;
+  B200_TRY(timestep_embedding(w, t, s->num_embed > 0 ? w->y_table : nullptr, y, s->num_embed, n, D, tfreq, th, c, stream));
+  B200_PROF(PROF_OTHER, launch_gemv(w->ada_w16, 16, s->dtype == B200_BF16, w->ada_b, c, mod, n, mod_rows, D, 1, 0, nullptr,
+                                    nullptr, 0, stream));
   return B200_OK;
 }
 
@@ -161,20 +284,16 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   B200_REQUIRE(!cfg || batch % 2 == 0, B200_ERR_SHAPE, "classifier-free guidance needs an even batch (got %d)", batch);
   B200_TRY(check_arch());
   Workspace ws;
-  carve(s, batch, workspace, &ws);
-  B200_REQUIRE(ws.bytes <= workspace_bytes, B200_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", ws.bytes,
-               workspace_bytes);
+  const size_t need = carve(s, batch, workspace, &ws);
+  B200_REQUIRE(need <= workspace_bytes, B200_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+  const BlockWeights stack{w->qkv_w16, w->qkv_w8, w->qkv_ws, w->qkv_b, w->proj_w16, w->proj_b,
+                           w->fc1_w16, w->fc1_w8, w->fc1_ws, w->fc1_b, w->fc2_w16, w->fc2_b};
+  B200_TRY(e4m3_stacks_ok("", stack));
 
-  const int D = s->hidden, H = s->heads, hd = D / H, F = s->frames, depth = s->depth;
+  const int D = s->hidden, F = s->frames, depth = s->depth;
   const int grid = s->input_size / s->patch, N = grid * grid;
-  const int T = batch * F * N;
-  const int rows_per_batch = F * N;
   const int bf16 = s->dtype == B200_BF16;
   const long long mod_bs = static_cast<long long>(depth) * 6 * D + 2 * D;
-  const int HID = s->mlp_hidden;
-  B200_REQUIRE((!w->qkv_w8 || w->qkv_ws) && (!w->fc1_w8 || w->fc1_ws), B200_ERR_SHAPE, "e4m3 weights need their scales");
-  B200_REQUIRE((w->qkv_w8 || w->qkv_w16) && (w->fc1_w8 || w->fc1_w16), B200_ERR_SHAPE,
-               "qkv and fc1 need a 16-bit or an e4m3 weight copy");
 
   // stream-K ordering flags: zero at the start of the step (every stream-K GEMM leaves them zero again; this memset only
   // makes the step independent of whatever the workspace held before -- a fresh allocation, an aborted run)
@@ -186,37 +305,14 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   B200_PROF(PROF_OTHER, launch_patch_embed(x, cfg ? batch / 2 : batch, w->patch_w, w->patch_b, w->pos_embed, ws.x, batch, F,
                               s->in_channels, s->input_size, s->patch, D, 0, stream));
 
-  // ---- blocks (latte.py:345-368); rows stay in (b, f, n) order for all of them
+  // ---- blocks (latte.py:345-368), alternately spatial and temporal; rows stay in (b, f, n) order for all of them
+  const Step st{ws.x, ws.h, ws.qkv, ws.g, ws.sk_flags, batch, F, N, s->heads, D, s->mlp_hidden, mod_bs, bf16, stream};
   for (int i = 0; i < depth; ++i) {
-    const float* m = ws.mod + static_cast<size_t>(i) * 6 * D;  // [shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp]
-    const uint16_t* proj_w = static_cast<const uint16_t*>(w->proj_w16) + static_cast<size_t>(i) * D * D;
-    const uint16_t* fc2_w = static_cast<const uint16_t*>(w->fc2_w16) + static_cast<size_t>(i) * D * HID;
-
-    B200_TRY(ln_modulate_linear(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->qkv_w16, w->qkv_w8, w->qkv_ws,
-                                w->qkv_b, i, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
-
-    AttnArgs aa{};
-    aa.qkv = ws.qkv; aa.out = ws.h; aa.batch = batch; aa.frames = F; aa.tokens = N; aa.heads = H; aa.head_dim = hd;
-    aa.bf16 = bf16; aa.temporal = i & 1;
-    B200_PROF(PROF_ATTN, launch_attention(aa, stream));
-
-    GemmArgs gp{};
-    gp.A = ws.h; gp.W = proj_w; gp.bias = w->proj_b + static_cast<size_t>(i) * D;
-    gp.M = T; gp.N = D; gp.K = D; gp.bf16 = bf16; gp.epilogue = B200_EPI_GATE_RESIDUAL; gp.resid = ws.x; gp.w_const = 1;
-    gp.gate = m + 2 * D; gp.gate_batch_stride = mod_bs; gp.rows_per_batch = rows_per_batch; gp.sk_flags = ws.sk_flags;
-    B200_PROF(PROF_GEMM, launch_gemm(gp, stream));
-
-    B200_TRY(ln_modulate_linear(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->fc1_w16, w->fc1_w8, w->fc1_ws,
-                                w->fc1_b, i, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
-
-    GemmArgs g2{};
-    g2.A = ws.g; g2.W = fc2_w; g2.bias = w->fc2_b + static_cast<size_t>(i) * D;
-    g2.M = T; g2.N = D; g2.K = HID; g2.bf16 = bf16; g2.epilogue = B200_EPI_GATE_RESIDUAL; g2.resid = ws.x; g2.w_const = 1;
-    g2.gate = m + 5 * D; g2.gate_batch_stride = mod_bs; g2.rows_per_batch = rows_per_batch; g2.sk_flags = ws.sk_flags;
-    if (i == 0) {  // x = x + temp_embed before the first temporal block (latte.py:357-358), folded into block 0's last epilogue
-      g2.row_add = w->temp_embed; g2.row_add_div = N; g2.row_add_period = F;
-    }
-    B200_PROF(PROF_GEMM, launch_gemm(g2, stream));
+    const float* m = ws.mod + static_cast<size_t>(i) * 6 * D;
+    const BlockWeights b = layer(stack, i, D, s->mlp_hidden);
+    B200_TRY(attention_half(st, b, m, i & 1));
+    // x = x + temp_embed before the first temporal block (latte.py:357-358), folded into block 0's last epilogue
+    B200_TRY(mlp_half(st, b, m, i == 0 ? w->temp_embed : nullptr));
   }
 
   // ---- final layer + unpatchify (latte.py:374-376), then guidance (latte.py:394-398)
@@ -231,7 +327,6 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   return B200_OK;
 }
 
-
 // ====================================================================================================== LatteT2V
 struct T2VWorkspace {
   float* x; uint16_t* h; uint16_t* qkv; uint16_t* g;
@@ -239,52 +334,41 @@ struct T2VWorkspace {
   float* ones; float* tfreq; float* th; float* emb; float* ts; float* mod;
   unsigned long long* sk_flags;
   float* head;
-  size_t bytes;
 };
 
 int t2v_shape_ok(const B200T2VShape* s, int batch, int text_len) {
-  B200_REQUIRE(s != nullptr && batch > 0, B200_ERR_SHAPE, "t2v: bad shape/batch");
-  B200_REQUIRE(s->layers > 0 && s->heads > 0 && s->hidden % s->heads == 0, B200_ERR_SHAPE, "t2v: hidden %d / heads %d", s->hidden, s->heads);
-  const int hd = s->hidden / s->heads;
-  B200_REQUIRE(hd == 64 || hd == 72 || hd == 80, B200_ERR_UNSUPPORTED, "t2v: head_dim %d unsupported", hd);
-  B200_REQUIRE(s->hidden % 64 == 0 && s->mlp_hidden % 64 == 0 && s->caption_channels % 64 == 0, B200_ERR_UNSUPPORTED,
-               "t2v: hidden, mlp_hidden, caption_channels must be multiples of 64");
-  B200_REQUIRE(s->patch == 2 && s->input_size % 2 == 0, B200_ERR_UNSUPPORTED, "t2v: patch size %d not built", s->patch);
+  B200_TRY(block_shape_ok("t2v: ", s, batch));
+  B200_REQUIRE(s->layers > 0, B200_ERR_SHAPE, "t2v: layers %d must be positive", s->layers);
+  B200_REQUIRE(s->caption_channels % 64 == 0, B200_ERR_UNSUPPORTED, "t2v: caption_channels %d must be a multiple of 64",
+               s->caption_channels);
   B200_REQUIRE(text_len >= 1 && text_len <= 128, B200_ERR_UNSUPPORTED, "t2v: text length %d (1..128 built)", text_len);
-  B200_REQUIRE(s->dtype == B200_FP16 || s->dtype == B200_BF16, B200_ERR_DTYPE, "t2v: dtype %d unknown", s->dtype);
-  B200_REQUIRE(s->out_channels * 4 <= 32, B200_ERR_UNSUPPORTED, "t2v: p*p*out_channels > 32");
-  const int grid = s->input_size / 2;
+  const int grid = s->input_size / s->patch;
   B200_REQUIRE((s->frames * grid * grid) % 128 == 0, B200_ERR_UNSUPPORTED, "t2v: tokens per sample must be a multiple of 128");
   return B200_OK;
 }
 
-void t2v_carve(const B200T2VShape* s, int batch, int text_len, void* base, T2VWorkspace* ws) {
+size_t t2v_carve(const B200T2VShape* s, int batch, int text_len, void* base, T2VWorkspace* ws) {
   const size_t grid = s->input_size / s->patch;
-  const size_t T = static_cast<size_t>(batch) * s->frames * grid * grid;
-  const size_t D = s->hidden, R = static_cast<size_t>(batch) * text_len;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    void* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
-    off += align_up(bytes, 1024);
-    return p;
-  };
-  ws->x = static_cast<float*>(take(T * D * 4));
-  ws->h = static_cast<uint16_t*>(take(T * D * 2));
-  ws->qkv = static_cast<uint16_t*>(take(T * 3 * D * 2));
-  ws->g = static_cast<uint16_t*>(take(T * static_cast<size_t>(s->mlp_hidden) * 2));
-  ws->text16 = static_cast<uint16_t*>(take(R * s->caption_channels * 2));
-  ws->cap_h = static_cast<uint16_t*>(take(R * D * 2));
-  ws->cap_o = static_cast<uint16_t*>(take(R * D * 2));
-  ws->kv_all = static_cast<uint16_t*>(take(R * static_cast<size_t>(s->layers) * 2 * D * 2));
-  ws->ones = static_cast<float*>(take(D * 4));
-  ws->tfreq = static_cast<float*>(take(static_cast<size_t>(batch) * 256 * 4));
-  ws->th = static_cast<float*>(take(static_cast<size_t>(batch) * D * 4));
-  ws->emb = static_cast<float*>(take(static_cast<size_t>(batch) * D * 4));
-  ws->ts = static_cast<float*>(take(static_cast<size_t>(batch) * 6 * D * 4));
-  ws->mod = static_cast<float*>(take(static_cast<size_t>(batch) * (static_cast<size_t>(s->layers) * 2 * 6 * D + 2 * D) * 4));
-  ws->sk_flags = static_cast<unsigned long long*>(take(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8));
-  ws->head = static_cast<float*>(take((T + 1) * 32 * 4));
-  ws->bytes = off;
+  const size_t B = batch, T = B * s->frames * grid * grid;
+  const size_t D = s->hidden, R = B * text_len;
+  Arena a{static_cast<uint8_t*>(base)};
+  ws->x = a.take<float>(T * D * 4);
+  ws->h = a.take<uint16_t>(T * D * 2);
+  ws->qkv = a.take<uint16_t>(T * 3 * D * 2);
+  ws->g = a.take<uint16_t>(T * s->mlp_hidden * 2);
+  ws->text16 = a.take<uint16_t>(R * s->caption_channels * 2);
+  ws->cap_h = a.take<uint16_t>(R * D * 2);
+  ws->cap_o = a.take<uint16_t>(R * D * 2);
+  ws->kv_all = a.take<uint16_t>(R * s->layers * 2 * D * 2);
+  ws->ones = a.take<float>(D * 4);
+  ws->tfreq = a.take<float>(B * 256 * 4);
+  ws->th = a.take<float>(B * D * 4);
+  ws->emb = a.take<float>(B * D * 4);
+  ws->ts = a.take<float>(B * 6 * D * 4);
+  ws->mod = a.take<float>(B * (s->layers * 2 * 6 * D + 2 * D) * 4);
+  ws->sk_flags = a.take<unsigned long long>(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8);
+  ws->head = a.take<float>((T + 1) * 32 * 4);
+  return a.off;
 }
 
 int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, const int64_t* t, const float* text,
@@ -295,108 +379,64 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   B200_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 1023) == 0, B200_ERR_ALIGN, "t2v: workspace must be 1024-byte aligned");
   B200_TRY(check_arch());
   T2VWorkspace ws;
-  t2v_carve(s, batch, text_len, workspace, &ws);
-  B200_REQUIRE(ws.bytes <= workspace_bytes, B200_ERR_WORKSPACE, "t2v: workspace too small: need %zu bytes, got %zu", ws.bytes, workspace_bytes);
+  const size_t need = t2v_carve(s, batch, text_len, workspace, &ws);
+  B200_REQUIRE(need <= workspace_bytes, B200_ERR_WORKSPACE, "t2v: workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+  const BlockWeights spatial{w->s_qkv_w16, w->s_qkv_w8, w->s_qkv_ws, w->s_qkv_b, w->s_out_w16, w->s_out_b,
+                             w->s_fc1_w16, w->s_fc1_w8, w->s_fc1_ws, w->s_fc1_b, w->s_fc2_w16, w->s_fc2_b};
+  const BlockWeights temporal{w->t_qkv_w16, w->t_qkv_w8, w->t_qkv_ws, w->t_qkv_b, w->t_out_w16, w->t_out_b,
+                              w->t_fc1_w16, w->t_fc1_w8, w->t_fc1_ws, w->t_fc1_b, w->t_fc2_w16, w->t_fc2_b};
+  B200_TRY(e4m3_stacks_ok("t2v: s_", spatial));
+  B200_TRY(e4m3_stacks_ok("t2v: t_", temporal));
 
-  const int D = s->hidden, H = s->heads, hd = D / H, F = s->frames, L = s->layers, HID = s->mlp_hidden;
+  const int D = s->hidden, H = s->heads, F = s->frames, L = s->layers, HID = s->mlp_hidden;
   const int grid = s->input_size / s->patch, N = grid * grid;
   const int T = batch * F * N, R = batch * text_len;
-  const int rows_per_batch = F * N;
   const int bf16 = s->dtype == B200_BF16;
   const long long mod_bs = static_cast<long long>(L) * 2 * 6 * D + 2 * D;
-  B200_REQUIRE((!w->s_qkv_w8 || w->s_qkv_ws) && (!w->s_fc1_w8 || w->s_fc1_ws) && (!w->t_qkv_w8 || w->t_qkv_ws) &&
-                   (!w->t_fc1_w8 || w->t_fc1_ws),
-               B200_ERR_SHAPE, "t2v: e4m3 weights need their scales");
-  B200_REQUIRE((w->s_qkv_w8 || w->s_qkv_w16) && (w->s_fc1_w8 || w->s_fc1_w16) && (w->t_qkv_w8 || w->t_qkv_w16) &&
-                   (w->t_fc1_w8 || w->t_fc1_w16),
-               B200_ERR_SHAPE, "t2v: qkv and fc1 need a 16-bit or an e4m3 weight copy");
 
   B200_CHECK_CUDA(cudaMemsetAsync(ws.sk_flags, 0, static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8, stream));
   // ---- conditioning (latte_t2v.py:782-784): emb = TimestepEmbedding(sincos(t)); ts = Linear(SiLU(emb)); tables + ts
-  B200_PROF(PROF_OTHER, launch_timestep_freq(reinterpret_cast<const long long*>(t), ws.tfreq, batch, stream));
-  B200_PROF(PROF_OTHER, launch_gemv(w->t_w0, 32, 0, w->t_b0, ws.tfreq, ws.th, batch, D, 256, 0, 1, nullptr, nullptr, 0, stream));
-  B200_PROF(PROF_OTHER, launch_gemv(w->t_w2, 32, 0, w->t_b2, ws.th, ws.emb, batch, D, D, 0, 0, nullptr, nullptr, 0, stream));
+  B200_TRY(timestep_embedding(w, t, nullptr, nullptr, 0, batch, D, ws.tfreq, ws.th, ws.emb, stream));
   B200_PROF(PROF_OTHER, launch_gemv(w->ada_w16, 16, bf16, w->ada_b, ws.emb, ws.ts, batch, 6 * D, D, 1, 0, nullptr, nullptr, 0, stream));
   B200_PROF(PROF_OTHER, launch_t2v_mod(w->tables, ws.ts, w->final_table, ws.emb, ws.mod, batch, 2 * L, D, stream));
   B200_PROF(PROF_OTHER, launch_fill(ws.ones, 1.0f, D, stream));
 
   // ---- text: caption projection once per sample (latte_t2v.py:789), then K/V of EVERY layer's cross-attention in one GEMM
   B200_PROF(PROF_OTHER, launch_cast16(text, ws.text16, static_cast<long long>(R) * s->caption_channels, bf16, stream));
-  {
-    GemmArgs a{};
-    a.A = ws.text16; a.W = w->cap_w1_16; a.bias = w->cap_b1; a.M = R; a.N = D; a.K = s->caption_channels; a.bf16 = bf16;
-    a.epilogue = B200_EPI_BIAS_GELU; a.out16 = ws.cap_h;
-    B200_PROF(PROF_GEMM, launch_gemm(a, stream));
-    GemmArgs b{};
-    b.A = ws.cap_h; b.W = w->cap_w2_16; b.bias = w->cap_b2; b.M = R; b.N = D; b.K = D; b.bf16 = bf16;
-    b.epilogue = B200_EPI_BIAS; b.out16 = ws.cap_o;
-    B200_PROF(PROF_GEMM, launch_gemm(b, stream));
-    GemmArgs c{};
-    c.A = ws.cap_o; c.W = w->c_kv_w16; c.bias = w->c_kv_b; c.M = R; c.N = L * 2 * D; c.K = D; c.bf16 = bf16;
-    c.epilogue = B200_EPI_BIAS; c.out16 = ws.kv_all;
-    B200_PROF(PROF_GEMM, launch_gemm(c, stream));
-  }
+  B200_PROF(PROF_GEMM, linear16(ws.text16, w->cap_w1_16, w->cap_b1, R, D, s->caption_channels, bf16, B200_EPI_BIAS_GELU, ws.cap_h, stream));
+  B200_PROF(PROF_GEMM, linear16(ws.cap_h, w->cap_w2_16, w->cap_b2, R, D, D, bf16, B200_EPI_BIAS, ws.cap_o, stream));
+  B200_PROF(PROF_GEMM, linear16(ws.cap_o, w->c_kv_w16, w->c_kv_b, R, L * 2 * D, D, bf16, B200_EPI_BIAS, ws.kv_all, stream));
 
   // ---- patch embedding + pos_embed (latte_t2v.py:731,773); x arrives as (b c f h w)
   B200_PROF(PROF_OTHER, launch_patch_embed(x, batch, w->patch_w, w->patch_b, w->pos_embed, ws.x, batch, F, s->in_channels,
                                            s->input_size, s->patch, D, 1, stream));
 
-  auto linear16 = [&](const void* A, const void* W, const float* bias, int M, int Nn, int K, int epi, void* o16) {
-    GemmArgs a{};
-    a.A = A; a.W = W; a.bias = bias; a.M = M; a.N = Nn; a.K = K; a.bf16 = bf16; a.epilogue = epi; a.out16 = o16; a.w_const = 1;
-    return launch_gemm(a, stream);
-  };
-  auto linear_resid = [&](const void* A, const void* W, const float* bias, int K, const float* gate, long long gate_bs,
-                          const float* row_add) {
-    GemmArgs a{};
-    a.A = A; a.W = W; a.bias = bias; a.M = T; a.N = D; a.K = K; a.bf16 = bf16; a.epilogue = B200_EPI_GATE_RESIDUAL; a.w_const = 1;
-    a.resid = ws.x; a.gate = gate; a.gate_batch_stride = gate_bs; a.rows_per_batch = rows_per_batch; a.sk_flags = ws.sk_flags;
-    if (row_add) { a.row_add = row_add; a.row_add_div = N; a.row_add_period = F; }
-    return launch_gemm(a, stream);
-  };
+  const Step st{ws.x, ws.h, ws.qkv, ws.g, ws.sk_flags, batch, F, N, H, D, HID, mod_bs, bf16, stream};
   const size_t DD = static_cast<size_t>(D) * D;
-
   for (int l = 0; l < L; ++l) {
     // ------------------------------------------------ spatial block (diffusers BasicTransformerBlock; latte_t2v.py:862-870)
     const float* m = ws.mod + static_cast<size_t>(2 * l) * 6 * D;
-    B200_TRY(ln_modulate_linear(ws.x, m + 0 * D, m + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->s_qkv_w16, w->s_qkv_w8,
-                                w->s_qkv_ws, w->s_qkv_b, l, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
-    AttnArgs aa{};
-    aa.qkv = ws.qkv; aa.out = ws.h; aa.batch = batch; aa.frames = F; aa.tokens = N; aa.heads = H; aa.head_dim = hd; aa.bf16 = bf16;
-    aa.temporal = 0;
-    B200_PROF(PROF_ATTN, launch_attention(aa, stream));
-    B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->s_out_w16) + l * DD, w->s_out_b + static_cast<size_t>(l) * D, D,
-                                      m + 2 * D, mod_bs, nullptr));
+    const BlockWeights sb = layer(spatial, l, D, HID);
+    B200_TRY(attention_half(st, sb, m, 0));
     // cross-attention on the UN-normalised stream (no norm2 before attn2 in ada_norm_single mode), residual without gate
     B200_PROF(PROF_OTHER, launch_cast16(ws.x, ws.h, static_cast<long long>(T) * D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->c_q_w16) + l * DD, w->c_q_b + static_cast<size_t>(l) * D, T, D, D,
-                                  B200_EPI_BIAS, ws.qkv));
+    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->c_q_w16) + l * DD, w->c_q_b + static_cast<size_t>(l) * D, T, D,
+                                  D, bf16, B200_EPI_BIAS, ws.qkv, stream));
     CrossAttnArgs ca{};
-    ca.q = ws.qkv; ca.kv = ws.kv_all + static_cast<size_t>(l) * 2 * D; ca.out = ws.h; ca.batch = batch; ca.q_rows_per_batch = rows_per_batch;
-    ca.kv_len = text_len; ca.q_row_stride = D; ca.kv_row_stride = L * 2 * D; ca.heads = H; ca.head_dim = hd; ca.bf16 = bf16;
+    ca.q = ws.qkv; ca.kv = ws.kv_all + static_cast<size_t>(l) * 2 * D; ca.out = ws.h; ca.batch = batch; ca.q_rows_per_batch = F * N;
+    ca.kv_len = text_len; ca.q_row_stride = D; ca.kv_row_stride = L * 2 * D; ca.heads = H; ca.head_dim = D / H; ca.bf16 = bf16;
     ca.key_bias = text_bias;     // padded prompts: (1 - mask) * -10000 per text token (latte_t2v.py:766-771), or NULL
     B200_PROF(PROF_ATTN, launch_cross_attention(ca, stream));
-    B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->c_out_w16) + l * DD, w->c_out_b + static_cast<size_t>(l) * D, D,
-                                      ws.ones, 0, nullptr));
-    B200_TRY(ln_modulate_linear(ws.x, m + 3 * D, m + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->s_fc1_w16, w->s_fc1_w8,
-                                w->s_fc1_ws, w->s_fc1_b, l, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
+    B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->c_out_w16) + l * DD, w->c_out_b + static_cast<size_t>(l) * D,
+                                      T, D, D, bf16, ws.x, ws.ones, 0, F * N, ws.sk_flags, stream));
     // + temp_pos_embed before the first temporal block (latte_t2v.py:894-895), folded into this epilogue
-    B200_PROF(PROF_GEMM, linear_resid(ws.g, static_cast<const uint16_t*>(w->s_fc2_w16) + static_cast<size_t>(l) * D * HID,
-                                      w->s_fc2_b + static_cast<size_t>(l) * D, HID, m + 5 * D, mod_bs,
-                                      (l == 0 && enable_temporal && F > 1) ? w->temp_embed : nullptr));
+    B200_TRY(mlp_half(st, sb, m, (l == 0 && enable_temporal && F > 1) ? w->temp_embed : nullptr));
     if (!enable_temporal) continue;
     // ------------------------------------------------ temporal block (BasicTransformerBlock_, latte_t2v.py:897-905)
     const float* mt = ws.mod + static_cast<size_t>(2 * l + 1) * 6 * D;
-    B200_TRY(ln_modulate_linear(ws.x, mt + 0 * D, mt + 1 * D, mod_bs, rows_per_batch, ws.h, T, D, w->t_qkv_w16, w->t_qkv_w8,
-                                w->t_qkv_ws, w->t_qkv_b, l, 3 * D, B200_EPI_BIAS, bf16, ws.qkv, stream));
-    aa.temporal = 1;
-    B200_PROF(PROF_ATTN, launch_attention(aa, stream));
-    B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->t_out_w16) + l * DD, w->t_out_b + static_cast<size_t>(l) * D, D,
-                                      mt + 2 * D, mod_bs, nullptr));
-    B200_TRY(ln_modulate_linear(ws.x, mt + 3 * D, mt + 4 * D, mod_bs, rows_per_batch, ws.h, T, D, w->t_fc1_w16, w->t_fc1_w8,
-                                w->t_fc1_ws, w->t_fc1_b, l, HID, B200_EPI_BIAS_GELU, bf16, ws.g, stream));
-    B200_PROF(PROF_GEMM, linear_resid(ws.g, static_cast<const uint16_t*>(w->t_fc2_w16) + static_cast<size_t>(l) * D * HID,
-                                      w->t_fc2_b + static_cast<size_t>(l) * D, HID, mt + 5 * D, mod_bs, nullptr));
+    const BlockWeights tb = layer(temporal, l, D, HID);
+    B200_TRY(attention_half(st, tb, mt, 1));
+    B200_TRY(mlp_half(st, tb, mt, nullptr));
   }
 
   // ---- output head (latte_t2v.py:918-936): table + embedded_timestep -> shift, scale; LN; modulate; proj_out; unpatchify to (b c f h w)
@@ -406,31 +446,9 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   return B200_OK;
 }
 
-int output_head(const float* x, uint16_t* h, float* head, const float* shift, const float* scale, long long mod_bs,
-                const float* w32, const void* w16, const float* bias, float* out, int batch, int F, int grid, int patch,
-                int out_ch, int D, int bf16, int channels_first, unsigned long long* sk_flags, cudaStream_t stream) {
-  const int n_out = patch * patch * out_ch;
-  const int T = batch * F * grid * grid;
-  if (w16 == nullptr || n_out != 32) {
-    B200_PROF(PROF_OTHER, launch_final_layer(x, shift, scale, mod_bs, w32, bias, out, batch, F, grid, patch, out_ch, D, channels_first, stream));
-    return B200_OK;
-  }
-  float* ones = head + static_cast<size_t>(T) * 32;
-  B200_CHECK_CUDA(cudaMemsetAsync(head, 0, static_cast<size_t>(T) * 32 * 4, stream));
-  B200_PROF(PROF_OTHER, launch_fill(ones, 1.0f, 32, stream));
-  B200_PROF(PROF_LN, launch_ln_modulate(x, shift, scale, mod_bs, F * grid * grid, h, T, D, bf16, stream));
-  GemmArgs g{};
-  g.A = h; g.W = w16; g.bias = bias; g.M = T; g.N = n_out; g.K = D; g.bf16 = bf16; g.epilogue = B200_EPI_GATE_RESIDUAL; g.w_const = 1;
-  g.resid = head; g.gate = ones; g.gate_batch_stride = 0; g.rows_per_batch = T; g.sk_flags = sk_flags;
-  B200_PROF(PROF_GEMM, launch_gemm(g, stream));
-  B200_PROF(PROF_OTHER, launch_unpatchify(head, out, batch, F, grid, patch, out_ch, channels_first, stream));
-  return B200_OK;
-}
-
 // ====================================================================================================== T5 encoder
 struct T5Workspace {
   float* x; uint16_t* h; uint16_t* qkv; uint16_t* att; uint16_t* g0; uint16_t* g; float* ones; unsigned long long* sk_flags;
-  size_t bytes;
 };
 
 int t5_shape_ok(const B200T5Shape* s, int batch) {
@@ -441,23 +459,18 @@ int t5_shape_ok(const B200T5Shape* s, int batch) {
   return B200_OK;
 }
 
-void t5_carve(const B200T5Shape* s, int batch, void* base, T5Workspace* ws) {
+size_t t5_carve(const B200T5Shape* s, int batch, void* base, T5Workspace* ws) {
   const size_t R = static_cast<size_t>(batch) * 128, D = s->d_model, I = static_cast<size_t>(s->heads) * 64, FF = s->d_ff;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    void* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
-    off += align_up(bytes, 1024);
-    return p;
-  };
-  ws->x = static_cast<float*>(take(R * D * 4));
-  ws->h = static_cast<uint16_t*>(take(R * D * 2));
-  ws->qkv = static_cast<uint16_t*>(take(R * 3 * I * 2));
-  ws->att = static_cast<uint16_t*>(take(R * I * 2));
-  ws->g0 = static_cast<uint16_t*>(take(R * FF * 2));
-  ws->g = static_cast<uint16_t*>(take(R * FF * 2));
-  ws->ones = static_cast<float*>(take(D * 4));
-  ws->sk_flags = static_cast<unsigned long long*>(take(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8));
-  ws->bytes = off;
+  Arena a{static_cast<uint8_t*>(base)};
+  ws->x = a.take<float>(R * D * 4);
+  ws->h = a.take<uint16_t>(R * D * 2);
+  ws->qkv = a.take<uint16_t>(R * 3 * I * 2);
+  ws->att = a.take<uint16_t>(R * I * 2);
+  ws->g0 = a.take<uint16_t>(R * FF * 2);
+  ws->g = a.take<uint16_t>(R * FF * 2);
+  ws->ones = a.take<float>(D * 4);
+  ws->sk_flags = a.take<unsigned long long>(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8);
+  return a.off;
 }
 
 // T5Stack.forward (encoder): embed -> [T5LayerSelfAttention, T5LayerFF] x layers -> final_layer_norm (transformers
@@ -470,24 +483,13 @@ int t5_encode(const B200T5Shape* s, const B200T5Weights* w, const int64_t* ids, 
   B200_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 1023) == 0, B200_ERR_ALIGN, "t5: workspace must be 1024-byte aligned");
   B200_TRY(check_arch());
   T5Workspace ws;
-  t5_carve(s, batch, workspace, &ws);
-  B200_REQUIRE(ws.bytes <= workspace_bytes, B200_ERR_WORKSPACE, "t5: workspace too small: need %zu bytes, got %zu", ws.bytes, workspace_bytes);
+  const size_t need = t5_carve(s, batch, workspace, &ws);
+  B200_REQUIRE(need <= workspace_bytes, B200_ERR_WORKSPACE, "t5: workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
   const int R = batch * 128, D = s->d_model, H = s->heads, I = H * 64, FF = s->d_ff;
   const int bf16 = s->dtype == B200_BF16;
   B200_CHECK_CUDA(cudaMemsetAsync(ws.sk_flags, 0, static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8, stream));
   B200_TRY(launch_fill(ws.ones, 1.0f, D, stream));
   B200_TRY(launch_embed(reinterpret_cast<const long long*>(ids), w->embed16, ws.x, R, D, s->vocab, bf16, stream));
-  auto linear16 = [&](const void* A, const void* W, int M, int N, int K, int epi, void* o16, const void* other) {
-    GemmArgs a{};
-    a.A = A; a.W = W; a.bias = nullptr; a.M = M; a.N = N; a.K = K; a.bf16 = bf16; a.epilogue = epi; a.out16 = o16; a.add16 = other; a.w_const = 1;
-    return launch_gemm(a, stream);
-  };
-  auto linear_resid = [&](const void* A, const void* W, int K) {
-    GemmArgs a{};
-    a.A = A; a.W = W; a.bias = nullptr; a.M = R; a.N = D; a.K = K; a.bf16 = bf16; a.epilogue = B200_EPI_GATE_RESIDUAL; a.w_const = 1;
-    a.resid = ws.x; a.gate = ws.ones; a.gate_batch_stride = 0; a.rows_per_batch = R; a.sk_flags = ws.sk_flags;
-    return launch_gemm(a, stream);
-  };
   for (int l = 0; l < s->layers; ++l) {
     const uint16_t* qkv_w = static_cast<const uint16_t*>(w->qkv_w16) + static_cast<size_t>(l) * 3 * I * D;
     const uint16_t* o_w = static_cast<const uint16_t*>(w->o_w16) + static_cast<size_t>(l) * D * I;
@@ -496,18 +498,18 @@ int t5_encode(const B200T5Shape* s, const B200T5Weights* w, const int64_t* ids, 
     const uint16_t* wo = static_cast<const uint16_t*>(w->wo_w16) + static_cast<size_t>(l) * D * FF;
     // ---- T5LayerSelfAttention: x += o(attention(q, k, v of T5LayerNorm(x)) with position bias + mask, NO 1/sqrt(d) scale)
     B200_TRY(launch_rms_norm(ws.x, w->ln0_w + static_cast<size_t>(l) * D, ws.h, nullptr, R, D, s->eps, bf16, stream));
-    B200_TRY(linear16(ws.h, qkv_w, R, 3 * I, D, B200_EPI_BIAS, ws.qkv, nullptr));
+    B200_TRY(linear16(ws.h, qkv_w, nullptr, R, 3 * I, D, bf16, B200_EPI_BIAS, ws.qkv, stream));
     CrossAttnArgs ca{};
     ca.q = ws.qkv; ca.kv = ws.qkv + I; ca.out = ws.att; ca.batch = batch; ca.q_rows_per_batch = 128; ca.kv_len = 128;
     ca.kv_batch_rows = 128; ca.q_row_stride = 3 * I; ca.kv_row_stride = 3 * I; ca.heads = H; ca.head_dim = 64; ca.bf16 = bf16;
     ca.key_bias = key_bias; ca.pos_bias = pos_bias; ca.scale = 1.0f;
     B200_TRY(launch_cross_attention(ca, stream));
-    B200_TRY(linear_resid(ws.att, o_w, I));
+    B200_TRY(linear_resid(ws.att, o_w, nullptr, R, D, I, bf16, ws.x, ws.ones, 0, R, ws.sk_flags, stream));
     // ---- T5LayerFF (gated-gelu): x += wo(gelu_new(wi_0 h) * wi_1 h), h = T5LayerNorm(x)
     B200_TRY(launch_rms_norm(ws.x, w->ln1_w + static_cast<size_t>(l) * D, ws.h, nullptr, R, D, s->eps, bf16, stream));
-    B200_TRY(linear16(ws.h, wi0, R, FF, D, B200_EPI_BIAS_GELU, ws.g0, nullptr));
-    B200_TRY(linear16(ws.h, wi1, R, FF, D, B200_EPI_BIAS_MUL16, ws.g, ws.g0));
-    B200_TRY(linear_resid(ws.g, wo, FF));
+    B200_TRY(linear16(ws.h, wi0, nullptr, R, FF, D, bf16, B200_EPI_BIAS_GELU, ws.g0, stream));
+    B200_TRY(linear16(ws.h, wi1, nullptr, R, FF, D, bf16, B200_EPI_BIAS_MUL16, ws.g, stream, ws.g0));
+    B200_TRY(linear_resid(ws.g, wo, nullptr, R, D, FF, bf16, ws.x, ws.ones, 0, R, ws.sk_flags, stream));
   }
   B200_TRY(launch_rms_norm(ws.x, w->final_w, nullptr, out, R, D, s->eps, bf16, stream));
   return B200_OK;
@@ -526,8 +528,7 @@ B200_API int b200_frames_to_uint8(const void* video, int dtype, int n, int c, in
 B200_API size_t b200_t5_workspace_bytes(const B200T5Shape* shape, int batch) {
   if (b200::t5_shape_ok(shape, batch) != B200_OK) return 0;
   b200::T5Workspace ws;
-  b200::t5_carve(shape, batch, nullptr, &ws);
-  return ws.bytes;
+  return b200::t5_carve(shape, batch, nullptr, &ws);
 }
 
 B200_API int b200_t5_encode(const B200T5Shape* shape, const B200T5Weights* w, const int64_t* ids, const float* key_bias,
@@ -587,8 +588,7 @@ B200_API int b200_abi_version(void) { return B200_ABI_VERSION; }
 B200_API size_t b200_latte_workspace_bytes(const B200LatteShape* shape, int batch) {
   if (b200::shape_ok(shape, batch) != B200_OK) return 0;
   b200::Workspace ws;
-  b200::carve(shape, batch, nullptr, &ws);
-  return ws.bytes;
+  return b200::carve(shape, batch, nullptr, &ws);
 }
 
 B200_API int b200_latte_forward(const B200LatteShape* shape, const B200LatteWeights* w, const float* x, const int64_t* t,
@@ -618,10 +618,10 @@ B200_API int b200_latte_conditioning(const B200LatteShape* shape, const B200Latt
                "workspace and mod_out must be 1024-byte aligned");
   B200_REQUIRE(workspace_bytes >= b200::conditioning_scratch_bytes(shape, n), B200_ERR_WORKSPACE, "conditioning workspace too small");
   B200_TRY(b200::check_arch());
-  uint8_t* base = static_cast<uint8_t*>(workspace);
-  float* tfreq = reinterpret_cast<float*>(base);
-  float* th = reinterpret_cast<float*>(base + b200::align_up(static_cast<size_t>(n) * 256 * 4, 1024));
-  float* c = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(th) + b200::align_up(static_cast<size_t>(n) * shape->hidden * 4, 1024));
+  b200::Arena a{static_cast<uint8_t*>(workspace)};
+  float* tfreq = a.take<float>(static_cast<size_t>(n) * 256 * 4);
+  float* th = a.take<float>(static_cast<size_t>(n) * shape->hidden * 4);
+  float* c = a.take<float>(static_cast<size_t>(n) * shape->hidden * 4);
   return b200::conditioning(shape, w, t, y, n, tfreq, th, c, mod_out, static_cast<cudaStream_t>(stream));
 }
 
@@ -658,8 +658,7 @@ B200_API int b200_attention(const void* qkv, void* out, int batch, int frames, i
 B200_API size_t b200_t2v_workspace_bytes(const B200T2VShape* shape, int batch, int text_len) {
   if (b200::t2v_shape_ok(shape, batch, text_len) != B200_OK) return 0;
   b200::T2VWorkspace ws;
-  b200::t2v_carve(shape, batch, text_len, nullptr, &ws);
-  return ws.bytes;
+  return b200::t2v_carve(shape, batch, text_len, nullptr, &ws);
 }
 
 B200_API int b200_t2v_forward(const B200T2VShape* shape, const B200T2VWeights* w, const float* x, const int64_t* t,
@@ -731,7 +730,7 @@ B200_API int b200_linear_gelu_both(const void* A, const void* W, const float* bi
   B200_DT(dtype);
   b200::GemmArgs a{};
   a.A = A; a.W = W; a.bias = bias; a.M = M; a.N = N; a.K = K; a.bf16 = dtype == B200_BF16; a.epilogue = B200_EPI_BIAS_GELU_BOTH;
-  a.out16 = u16; a.out16b = a16; a.w_const = 1;
+  a.out16 = u16; a.out16b = a16;
   return b200::launch_gemm(a, static_cast<cudaStream_t>(stream));
 }
 B200_API int b200_transpose16(const void* in16, void* out16, int rows, int cols, void* stream) {

@@ -98,8 +98,6 @@ struct GemmArgs {
   const float* row_add; // optional [period, N] fp32 added to resid rows: row_add[((row / row_add_div) % row_add_period) * N + col]
   int row_add_div, row_add_period;
   int block_n;          // 0 = auto
-  int w_const;          // 1: W is a constant weight matrix (never written during the step); a scheduling hint the
-                        // current kernel does not need (every operand is fetched after the grid dependency resolves)
   int mn_major;         // bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (N % 128 == 0).  3 = wgrad (dW[M, N] += dY[K, M]^T X[K, N]),
                         // 2 = dgrad (dX[M, N] = dY[M, K] W[K, N] with the weight in its nn.Linear [out, in] layout);
                         // 1 is rejected (no caller transposes A alone)

@@ -23,6 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .ops import quantize_rows_e4m3
 from ._cache import DeviceCacheMixin
 from .training import GradientCheckpointingMixin
 
@@ -272,13 +273,8 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             # blocks like the 16-bit copies, then fc1; one scale per output channel (b200_quantize_rows_e4m3)
             w32 = torch.cat([b.attn.qkv.weight.detach() for b in blocks] + [b.mlp.fc1.weight.detach() for b in blocks]).to(
                 device=dev, dtype=torch.float32).contiguous()
-            rows, nq = w32.shape[0], self.depth * 3 * D
-            q8 = torch.empty(rows, D, dtype=torch.uint8, device=dev)
-            ws8 = torch.empty(rows, dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                rc = _lib.load().b200_quantize_rows_e4m3(w32.data_ptr(), rows, D, q8.data_ptr(), ws8.data_ptr(),
-                                                         torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(rc, "b200_quantize_rows_e4m3")
+            q8, ws8 = quantize_rows_e4m3(w32)
+            q8, nq = q8.view(torch.uint8), self.depth * 3 * D
             T["qkv_w8"], T["fc1_w8"] = q8[:nq], q8[nq:]
             T["qkv_ws"], T["fc1_ws"] = ws8[:nq], ws8[nq:]
 
@@ -296,16 +292,24 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         self._packed_key = key
         return self._packed
 
-    def _get_workspace(self, shape, batch, device):
-        lib = _lib.load()
-        need = lib.b200_latte_workspace_bytes(C.byref(shape), batch)
-        if need == 0:
-            raise RuntimeError("latte_b200: unsupported configuration: " + _lib.last_error())
-        ws = self._workspace
-        if ws is None or ws.numel() < need or ws.device != device:
-            ws = torch.empty(need + 1024, dtype=torch.uint8, device=device)
-            self._workspace = ws
-        return ws, need
+    def _check_input(self, x):
+        if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[2] != self.in_channels \
+                or x.shape[3] != self.input_size or x.shape[4] != self.input_size:
+            raise ValueError(f"x must be (B, {self.num_frames}, {self.in_channels}, {self.input_size}, {self.input_size}), got {tuple(x.shape)}")
+        if self.pos_embed.device != x.device:
+            raise RuntimeError(f"model is on {self.pos_embed.device}, input on {x.device}")
+
+    def _labels(self, y, B, dev):
+        """Class labels as int64 on `dev` (None unless extras == 2), with the reference's label dropout in training mode."""
+        if self.extras != 2:
+            return None
+        if y is None:
+            raise ValueError("class-conditional model (extras=2) needs labels y")
+        yy = y.detach().to(device=dev, dtype=torch.int64).contiguous()
+        if self.training and self.y_embedder.dropout_prob > 0:  # token_drop, latte.py:137-146
+            drop = torch.rand(B, device=dev) < self.y_embedder.dropout_prob
+            yy = torch.where(drop, torch.full_like(yy, self.y_embedder.num_classes), yy)
+        return yy
 
     def _run(self, x, t, y, use_cfg, cfg_scale, trajectory_step=None):
         if not x.is_cuda:
@@ -315,13 +319,9 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             if use_cfg or trajectory_step is not None:
                 raise NotImplementedError("latte_b200: forward_with_cfg / trajectory conditioning are sampling-only; train through forward()")
             return self._run_train(x, t, y)
-        if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[2] != self.in_channels \
-                or x.shape[3] != self.input_size or x.shape[4] != self.input_size:
-            raise ValueError(f"x must be (B, {self.num_frames}, {self.in_channels}, {self.input_size}, {self.input_size}), got {tuple(x.shape)}")
+        self._check_input(x)
         lib = _lib.load()
         dev = x.device
-        if self.pos_embed.device != dev:
-            raise RuntimeError(f"model is on {self.pos_embed.device}, input on {dev}")
         B = x.shape[0]
         with torch.cuda.device(dev):
             shape, w, _, od = self._pack()
@@ -329,29 +329,23 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             tt = t.detach().to(device=dev, dtype=torch.int64).contiguous()
             if tt.numel() != B:
                 raise ValueError("t must have one entry per batch row")
-            yy = None
-            if self.extras == 2:
-                if y is None:
-                    raise ValueError("class-conditional model (extras=2) needs labels y")
-                yy = y.detach().to(device=dev, dtype=torch.int64).contiguous()
-                if self.training and self.y_embedder.dropout_prob > 0:  # token_drop, latte.py:137-146
-                    drop = torch.rand(B, device=dev) < self.y_embedder.dropout_prob
-                    yy = torch.where(drop, torch.full_like(yy, self.y_embedder.num_classes), yy)
+            yy = self._labels(y, B, dev)
             traj = self._trajectory
             mod = None
             if trajectory_step is not None and traj is not None:
                 mod = traj[int(trajectory_step)]                    # [B, depth*6D + 2D] rows precomputed for this step
                 if mod.shape[0] != B or mod.device != dev:
                     raise ValueError("precomputed conditioning does not match this batch")
+            need = lib.b200_latte_workspace_bytes(C.byref(shape), B)
+            if need == 0:
+                raise RuntimeError("latte_b200: unsupported configuration: " + _lib.last_error())
             if (self.use_cuda_graphs and not torch.is_grad_enabled() and not torch.cuda.is_current_stream_capturing()
                     and not _lib.profiling_enabled()):
-                out = self._run_graphed(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, dev)
+                out = self._run_graphed(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev)
             else:
                 out = torch.empty(B, self.num_frames, self.out_channels, self.input_size, self.input_size,
                                   dtype=torch.float32, device=dev)
-                ws, need = self._get_workspace(shape, B, dev)
-                base = (ws.data_ptr() + 1023) // 1024 * 1024
-                self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, base, need,
+                self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need,
                              torch.cuda.current_stream(dev).cuda_stream)
         pd = self.blocks[0].attn.qkv.weight.dtype
         return out if pd == torch.float32 else out.to(pd)
@@ -365,30 +359,19 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         from . import training
         if self.use_fp8:
             raise NotImplementedError("latte_b200: FP8 is a sampling path; clear use_fp8 to train")
-        if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[2] != self.in_channels \
-                or x.shape[3] != self.input_size or x.shape[4] != self.input_size:
-            raise ValueError(f"x must be (B, {self.num_frames}, {self.in_channels}, {self.input_size}, {self.input_size}), got {tuple(x.shape)}")
+        self._check_input(x)
         dev = x.device
-        if self.pos_embed.device != dev:
-            raise RuntimeError(f"model is on {self.pos_embed.device}, input on {dev}")
         _lib.load()
         od, ops = training.native_backend(self, self.blocks[0].attn.qkv.weight.dtype)
         B = x.shape[0]
         tt = t.to(device=dev, dtype=torch.int64)
-        yy = None
-        if self.extras == 2:
-            if y is None:
-                raise ValueError("class-conditional model (extras=2) needs labels y")
-            yy = y.to(device=dev, dtype=torch.int64)
-            if self.y_embedder.dropout_prob > 0:                        # token_drop, latte.py:137-146
-                drop = torch.rand(B, device=dev) < self.y_embedder.dropout_prob
-                yy = torch.where(drop, torch.full_like(yy, self.y_embedder.num_classes), yy)
+        yy = self._labels(y, B, dev)
         with torch.autocast("cuda", enabled=False):
             c = training.conditioning(self, tt, yy)
             return training.train_forward(self, ops, od, x.float(), c)
 
     def _launch(self, lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, base, need, stream):
-        """ONE C-ABI call = the whole forward (203 kernel launches for XL/2) enqueued on `stream`."""
+        """ONE C-ABI call = the whole forward (206 kernel launches for XL/2 with CFG) enqueued on `stream`."""
         if mod is not None:
             rc = lib.b200_latte_forward_conditioned(C.byref(shape), C.byref(w), xf.data_ptr(), mod.data_ptr(), B, int(use_cfg),
                                                     float(cfg_scale), out.data_ptr(), base, need, stream)
@@ -399,7 +382,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
                                         out.data_ptr(), base, need, stream)
             _lib.check(rc, "b200_latte_forward")
 
-    def _run_graphed(self, lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, dev):
+    def _run_graphed(self, lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev):
         """CUDA-graph replay of the forward.  The C-ABI call neither allocates nor synchronises and keeps no host-side launch
         state, so its launch sequence can be captured once per call signature and replayed with the inputs copied into
         fixed buffers: the per-step host cost drops from ~200 launches to three small copies and one graph launch.
@@ -412,13 +395,10 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             self._graphs[key] = {"graph": None}
             out = torch.empty(B, self.num_frames, self.out_channels, self.input_size, self.input_size,
                               dtype=torch.float32, device=dev)
-            ws, need = self._get_workspace(shape, B, dev)
-            base = (ws.data_ptr() + 1023) // 1024 * 1024
-            self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, base, need,
+            self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need,
                          torch.cuda.current_stream(dev).cuda_stream)
             return out
         if st["graph"] is None:
-            need = lib.b200_latte_workspace_bytes(C.byref(shape), B)
             st["ws"] = torch.empty(need + 1024, dtype=torch.uint8, device=dev)     # this graph's own scratch
             st["x"], st["t"] = torch.empty_like(xf), torch.empty_like(tt)
             st["y"] = torch.empty_like(yy) if yy is not None else None

@@ -197,12 +197,8 @@ class T5EncoderModel(DeviceCacheMixin, nn.Module):
             need = lib.b200_t5_workspace_bytes(C.byref(shape), B)
             if need == 0:
                 raise RuntimeError("latte_b200: unsupported T5 configuration: " + _lib.last_error())
-            ws = self._workspace
-            if ws is None or ws.numel() < need + 1024 or ws.device != dev:
-                ws = self._workspace = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
-            base = (ws.data_ptr() + 1023) // 1024 * 1024
             rc = lib.b200_t5_encode(C.byref(shape), C.byref(w), ids.data_ptr(), bias.data_ptr(), pos.data_ptr(), B, out.data_ptr(),
-                                    base, need, torch.cuda.current_stream(dev).cuda_stream)
+                                    self._aligned_workspace(need, dev), need, torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(rc, "b200_t5_encode")
         pd = self.dtype
         res = out[:, :L].contiguous()

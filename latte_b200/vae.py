@@ -370,10 +370,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             need = lib.b200_vae_encode_workspace_bytes(C.byref(e), n, h, w)
             if need == 0:
                 raise RuntimeError("latte_b200: unsupported VAE encode configuration: " + _lib.last_error())
-            ws = self._workspace
-            if ws is None or ws.numel() < need + 1024 or ws.device != dev:
-                ws = self._workspace = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
-            base = (ws.data_ptr() + 1023) // 1024 * 1024
+            base = self._aligned_workspace(need, dev)
             rc = lib.b200_vae_encode(C.byref(e), xf.data_ptr(), n, h, w, moments.data_ptr(), base, need,
                                      torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(rc, "b200_vae_encode")
@@ -482,10 +479,7 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             need = lib.b200_vae_workspace_bytes(C.byref(d), n, h, w)
             if need == 0:
                 raise RuntimeError("latte_b200: unsupported VAE configuration: " + _lib.last_error())
-            ws = self._workspace
-            if ws is None or ws.numel() < need + 1024 or ws.device != dev:
-                ws = self._workspace = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
-            base = (ws.data_ptr() + 1023) // 1024 * 1024
+            base = self._aligned_workspace(need, dev)
             if self._temporal:
                 if num_frames is None:
                     raise ValueError("AutoencoderKLTemporalDecoder.decode needs num_frames")

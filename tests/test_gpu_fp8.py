@@ -20,6 +20,7 @@ Bounds, element by element against fp64 (tests/fp64_bounds.py conventions):
     XL/2 4.1 / 3.7 of those units.  The tolerance is FP8_TOL_FACTOR = 6 units: the worst measured value plus ~45 %
     for rounding that differs between GPUs (the residual GEMMs' stream-K splits follow the SM count).  The element-wise
     fp64 tests above carry the kernels' correctness; this one catches errors in how the model uses them."""
+import ctypes as C
 import math
 import os
 import re
@@ -229,6 +230,35 @@ def test_fp8_toggle_restores_the_16bit_output(golden_dir):
     assert not torch.equal(o8, want)
     for o in o16:
         assert torch.equal(o, want)
+
+
+def test_fp8_forward_rejects_bad_e4m3_pointers(golden_dir):
+    """b200_latte_forward checks the e4m3 fields of the QKV and fc1 stacks before any launch: a stack with e4m3 bytes but
+    no scales, or with neither copy, is B200_ERR_SHAPE (the check b200_t2v_forward runs on each of its four stacks)."""
+    from latte_b200 import _lib
+    g, net, (x, t, y) = _build(golden_dir, "latte_tiny64_2_b2.npz")
+    net.use_fp8 = True
+    with torch.no_grad():
+        good = net(x, t, y=y)
+    shape, w, _, _ = net._packed
+    dev = good.device
+    out = torch.zeros_like(good)
+    lib = _lib.load()
+    B = x.shape[0]
+    need = lib.b200_latte_workspace_bytes(C.byref(shape), B)
+    ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
+    base = (ws.data_ptr() + 1023) // 1024 * 1024
+    xf = x.float().contiguous()
+    for name in ("qkv", "fc1"):
+        for broken in (name + "_ws", name + "_w8"):
+            bad = _lib.LatteWeights.from_buffer_copy(w)
+            setattr(bad, broken, None)
+            rc = lib.b200_latte_forward(C.byref(shape), C.byref(bad), xf.data_ptr(), t.data_ptr(),
+                                        y.data_ptr(), B, 0, 0.0, out.data_ptr(), base, need,
+                                        torch.cuda.current_stream(dev).cuda_stream)
+            assert rc == -1, f"{broken} = NULL: rc {rc}"
+    torch.cuda.synchronize()
+    assert not out.any(), "a rejected call launched"
 
 
 def test_fp8_training_raises(golden_dir):
