@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 6
+#define B200_ABI_VERSION 7
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
 #else
@@ -50,13 +50,18 @@ typedef struct B200LatteShape {
   int32_t hidden;       /* D */
   int32_t heads;        /* H; head_dim = D / H must be 64 or in (64, 80] */
   int32_t mlp_hidden;   /* int(D * mlp_ratio) */
-  int32_t patch;        /* p (only 2 is built) */
+  int32_t patch;        /* p: 2; with wide_patch set also 4 or 8 */
   int32_t in_channels;  /* C */
   int32_t out_channels; /* 2C if learn_sigma else C */
   int32_t input_size;   /* latent H = W */
   int32_t frames;       /* F */
   int32_t num_embed;    /* rows of the label table (num_classes + 1); 0 when extras != 2 */
   int32_t dtype;        /* B200_FP16 / B200_BF16: tensor-core operand type of the packed weights */
+  int32_t wide_patch;   /* (appended in ABI v7) 0: the rules of ABI v6, patch 2 and p*p*out_channels <= 32 only;
+                           nonzero: patch 2, 4 or 8 (Latte-S/B/L/XL /4 and /8).  A head wider than 32 outputs
+                           (p*p*out_channels 64 .. 512, a multiple of 32) needs final_w16 and runs on the tensor cores;
+                           (input_size / patch)^2 must be a spatial length b200_attention takes (a divisor of 128, 128,
+                           or a multiple of 256), checked before anything is launched */
 } B200LatteShape;
 
 /* Packed weights (device pointers, torch-owned).  fp32 unless noted.  `*_w16` are 16-bit copies in

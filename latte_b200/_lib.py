@@ -10,7 +10,7 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buffer
 OK = 0
 FP16, BF16 = 0, 1
@@ -22,7 +22,7 @@ ERR_NAMES = {-1: "SHAPE", -2: "DTYPE", -3: "ALIGN", -4: "ARCH", -5: "WORKSPACE",
 class LatteShape(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "depth", "hidden", "heads", "mlp_hidden", "patch", "in_channels", "out_channels", "input_size",
-        "frames", "num_embed", "dtype")]
+        "frames", "num_embed", "dtype", "wide_patch")]
 
 
 WEIGHT_FIELDS = (

@@ -53,7 +53,7 @@ struct Arena {
   }
 };
 
-// ---- shape rules Latte and LatteT2V share: head_dim, the GEMM K tile, the patch size, the operand type and the head width.
+// ---- shape rules Latte and LatteT2V share: head_dim, the GEMM K tile, the patch grid, the operand type and the head width.
 // `who` prefixes the message ("" for Latte, "t2v: " for LatteT2V).
 template <class Shape>
 int block_shape_ok(const char* who, const Shape* s, int batch) {
@@ -64,10 +64,14 @@ int block_shape_ok(const char* who, const Shape* s, int batch) {
   B200_REQUIRE(hd == 64 || hd == 72 || hd == 80, B200_ERR_UNSUPPORTED, "%shead_dim %d unsupported", who, hd);
   B200_REQUIRE(s->hidden % 64 == 0 && s->mlp_hidden % 64 == 0, B200_ERR_UNSUPPORTED,
                "%shidden %d and mlp_hidden %d must be multiples of 64 (GEMM K tile)", who, s->hidden, s->mlp_hidden);
-  B200_REQUIRE(s->patch == 2, B200_ERR_UNSUPPORTED, "%spatch size %d not built (only 2)", who, s->patch);
-  B200_REQUIRE(s->input_size % s->patch == 0, B200_ERR_SHAPE, "%sinput_size %d not divisible by patch", who, s->input_size);
+  B200_REQUIRE(s->patch > 0 && s->input_size % s->patch == 0, B200_ERR_SHAPE, "%sinput_size %d not divisible by patch %d", who,
+               s->input_size, s->patch);
+  // checked here so that a grid the attention does not take fails before the forward launches anything
+  const int grid = s->input_size / s->patch;
+  B200_REQUIRE(attention_spatial_len_ok(grid * grid), B200_ERR_UNSUPPORTED,
+               "%s%d x %d patches per frame: spatial attention takes a divisor of 128, 128 or a multiple of 256 tokens", who, grid,
+               grid);
   B200_REQUIRE(s->dtype == B200_FP16 || s->dtype == B200_BF16, B200_ERR_DTYPE, "%sdtype %d unknown", who, s->dtype);
-  B200_REQUIRE(s->out_channels * s->patch * s->patch <= 32, B200_ERR_UNSUPPORTED, "%sp*p*out_channels > 32", who);
   return B200_OK;
 }
 
@@ -194,21 +198,33 @@ int mlp_half(const Step& s, const BlockWeights& b, const float* m, const float* 
   return B200_OK;
 }
 
-// ---- output head (latte.py:197-201,297-310,374-376): LayerNorm + modulate -> Linear(D, p*p*C_out) -> unpatchify.
-// With a 16-bit weight copy and p*p*C_out == 32 the Linear runs on the tensor cores: the GEMM's gated-residual epilogue on a
-// zeroed fp32 buffer with gate = 1 IS "fp32 out = acc + bias".  Otherwise the fp32 CUDA-core kernel.
+// ---- output head (latte.py:197-201,297-310,374-376): LayerNorm + modulate -> Linear(D, n_out = p*p*C_out) -> unpatchify.
+// With a 16-bit weight copy and n_out == 32, or any n_out > 32 (patch 4 and 8), the Linear runs on the tensor cores: the
+// GEMM's gated-residual epilogue on a zeroed fp32 buffer with gate = 1 IS "fp32 out = acc + bias".  n_out < 32, or 32
+// without a 16-bit copy, takes the fp32 CUDA-core kernel, which holds at most 32 outputs per token.
+int head_width(int patch, int out_ch) { return patch * patch * out_ch; }
+
+// `head` workspace: the fp32 [T, n_out] buffer and its n_out ones; never smaller than the 32-wide one of patch 2
+size_t head_floats(size_t T, int n_out) { return (T + 1) * (n_out > 32 ? n_out : 32); }
+
+int head_ok(const char* who, int n_out, const void* w16) {
+  B200_REQUIRE(n_out <= 32 || (n_out % 32 == 0 && w16 != nullptr), B200_ERR_UNSUPPORTED,
+               "%sp*p*out_channels = %d: a head wider than 32 needs a multiple of 32 and a 16-bit weight copy", who, n_out);
+  return B200_OK;
+}
+
 int output_head(const float* x, uint16_t* h, float* head, const float* shift, const float* scale, long long mod_bs,
                 const float* w32, const void* w16, const float* bias, float* out, int batch, int F, int grid, int patch,
                 int out_ch, int D, int bf16, int channels_first, unsigned long long* sk_flags, cudaStream_t stream) {
-  const int n_out = patch * patch * out_ch;
+  const int n_out = head_width(patch, out_ch);
   const int T = batch * F * grid * grid;
-  if (w16 == nullptr || n_out != 32) {
+  if (w16 == nullptr || n_out < 32) {
     B200_PROF(PROF_OTHER, launch_final_layer(x, shift, scale, mod_bs, w32, bias, out, batch, F, grid, patch, out_ch, D, channels_first, stream));
     return B200_OK;
   }
-  float* ones = head + static_cast<size_t>(T) * 32;
-  B200_CHECK_CUDA(cudaMemsetAsync(head, 0, static_cast<size_t>(T) * 32 * 4, stream));
-  B200_PROF(PROF_OTHER, launch_fill(ones, 1.0f, 32, stream));
+  float* ones = head + static_cast<size_t>(T) * n_out;
+  B200_CHECK_CUDA(cudaMemsetAsync(head, 0, static_cast<size_t>(T) * n_out * 4, stream));
+  B200_PROF(PROF_OTHER, launch_fill(ones, 1.0f, n_out, stream));
   B200_PROF(PROF_LN, launch_ln_modulate(x, shift, scale, mod_bs, F * grid * grid, h, T, D, bf16, stream));
   B200_PROF(PROF_GEMM, linear_resid(h, w16, bias, T, n_out, D, bf16, head, ones, 0, T, sk_flags, stream));
   B200_PROF(PROF_OTHER, launch_unpatchify(head, out, batch, F, grid, patch, out_ch, channels_first, stream));
@@ -226,11 +242,19 @@ struct Workspace {
   float* c;          // [B, D]   t_emb (+ y_emb)
   float* mod;        // [B, depth*6D + 2D]
   unsigned long long* sk_flags;   // [B200_GEMM_SK_FLAGS] stream-K ordering flags (zeroed at the start of every forward)
-  float* head;       // [T, 32]  fp32 output of the head GEMM (zeroed, then reduce-added into), followed by 32 ones (its "gate")
+  float* head;       // [T, n_out] fp32 output of the head GEMM (zeroed, then reduce-added into), then n_out ones (its "gate");
+                     // sized by head_floats
 };
 
 int shape_ok(const B200LatteShape* s, int batch) {
   B200_TRY(block_shape_ok("", s, batch));
+  if (s->wide_patch) {
+    B200_REQUIRE(s->patch == 2 || s->patch == 4 || s->patch == 8, B200_ERR_UNSUPPORTED, "patch size %d not built (2, 4, 8)",
+                 s->patch);
+  } else {   // the rules of ABI v6
+    B200_REQUIRE(s->patch == 2, B200_ERR_UNSUPPORTED, "patch size %d not built (only 2; 4 and 8 need wide_patch)", s->patch);
+    B200_REQUIRE(s->out_channels * s->patch * s->patch <= 32, B200_ERR_UNSUPPORTED, "p*p*out_channels > 32");
+  }
   B200_REQUIRE(s->depth > 0 && s->depth % 2 == 0, B200_ERR_SHAPE, "depth %d must be even (spatial/temporal pairs)", s->depth);
   return B200_OK;
 }
@@ -249,7 +273,7 @@ size_t carve(const B200LatteShape* s, int batch, void* base, Workspace* ws) {
   ws->c = a.take<float>(B * D * 4);
   ws->mod = a.take<float>(B * (s->depth * 6 * D + 2 * D) * 4);
   ws->sk_flags = a.take<unsigned long long>(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8);
-  ws->head = a.take<float>((T + 1) * 32 * 4);
+  ws->head = a.take<float>(head_floats(T, head_width(s->patch, s->out_channels)) * 4);
   return a.off;
 }
 
@@ -289,6 +313,7 @@ int forward(const B200LatteShape* s, const B200LatteWeights* w, const float* x, 
   const BlockWeights stack{w->qkv_w16, w->qkv_w8, w->qkv_ws, w->qkv_b, w->proj_w16, w->proj_b,
                            w->fc1_w16, w->fc1_w8, w->fc1_ws, w->fc1_b, w->fc2_w16, w->fc2_b};
   B200_TRY(e4m3_stacks_ok("", stack));
+  B200_TRY(head_ok("", head_width(s->patch, s->out_channels), w->final_w16));
 
   const int D = s->hidden, F = s->frames, depth = s->depth;
   const int grid = s->input_size / s->patch, N = grid * grid;
@@ -338,6 +363,8 @@ struct T2VWorkspace {
 
 int t2v_shape_ok(const B200T2VShape* s, int batch, int text_len) {
   B200_TRY(block_shape_ok("t2v: ", s, batch));
+  B200_REQUIRE(s->patch == 2, B200_ERR_UNSUPPORTED, "t2v: patch size %d not built (only 2)", s->patch);
+  B200_REQUIRE(s->out_channels * s->patch * s->patch <= 32, B200_ERR_UNSUPPORTED, "t2v: p*p*out_channels > 32");
   B200_REQUIRE(s->layers > 0, B200_ERR_SHAPE, "t2v: layers %d must be positive", s->layers);
   B200_REQUIRE(s->caption_channels % 64 == 0, B200_ERR_UNSUPPORTED, "t2v: caption_channels %d must be a multiple of 64",
                s->caption_channels);
@@ -367,7 +394,7 @@ size_t t2v_carve(const B200T2VShape* s, int batch, int text_len, void* base, T2V
   ws->ts = a.take<float>(B * 6 * D * 4);
   ws->mod = a.take<float>(B * (s->layers * 2 * 6 * D + 2 * D) * 4);
   ws->sk_flags = a.take<unsigned long long>(static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8);
-  ws->head = a.take<float>((T + 1) * 32 * 4);
+  ws->head = a.take<float>(head_floats(T, head_width(s->patch, s->out_channels)) * 4);
   return a.off;
 }
 
@@ -387,6 +414,7 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
                               w->t_fc1_w16, w->t_fc1_w8, w->t_fc1_ws, w->t_fc1_b, w->t_fc2_w16, w->t_fc2_b};
   B200_TRY(e4m3_stacks_ok("t2v: s_", spatial));
   B200_TRY(e4m3_stacks_ok("t2v: t_", temporal));
+  B200_TRY(head_ok("t2v: ", head_width(s->patch, s->out_channels), w->final_w16));
 
   const int D = s->hidden, H = s->heads, F = s->frames, L = s->layers, HID = s->mlp_hidden;
   const int grid = s->input_size / s->patch, N = grid * grid;

@@ -391,6 +391,10 @@ int launch_any(int mode, int bf16, bool tail, const CUtensorMap* m, const AttnDe
 
 }  // namespace
 
+bool attention_spatial_len_ok(int tokens) {
+  return tokens > 0 && (tokens >= 128 ? tokens == 128 || tokens % 256 == 0 : 128 % tokens == 0);
+}
+
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   B200_REQUIRE(a.batch > 0 && a.frames > 0 && a.tokens > 0 && a.heads > 0, B200_ERR_SHAPE, "attention: bad shape");
   B200_REQUIRE(a.head_dim == 64 || a.head_dim == 72 || a.head_dim == 80, B200_ERR_UNSUPPORTED,
@@ -420,14 +424,14 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   dim3 grid;
   if (!a.temporal) {
     if (a.tokens >= 128) {
-      B200_REQUIRE(a.tokens == 128 || a.tokens % 256 == 0, B200_ERR_UNSUPPORTED,
+      B200_REQUIRE(attention_spatial_len_ok(a.tokens), B200_ERR_UNSUPPORTED,
                    "attention: spatial sequence length %d unsupported (<=64 power of two, 128, multiples of 256)", a.tokens);
       mode = MODE_FULL;
       p.chunks = a.tokens / kChunk;
       p.tiles_per_seq = a.tokens / 128;
       grid = dim3(static_cast<unsigned>(a.batch * a.frames * p.tiles_per_seq), H);
     } else {
-      B200_REQUIRE(128 % a.tokens == 0, B200_ERR_UNSUPPORTED, "attention: spatial sequence length %d must divide 128", a.tokens);
+      B200_REQUIRE(attention_spatial_len_ok(a.tokens), B200_ERR_UNSUPPORTED, "attention: spatial sequence length %d must divide 128", a.tokens);
       mode = MODE_PACKED;
       p.group = a.tokens;
       p.gshift = ilog2(a.tokens);

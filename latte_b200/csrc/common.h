@@ -125,6 +125,8 @@ struct AttnArgs {
   int temporal;      // 0: sequences over tokens within a frame; 1: sequences over frames at a fixed token
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
+// spatial sequence lengths launch_attention takes: a divisor of 128, 128, or a multiple of 256
+bool attention_spatial_len_ok(int tokens);
 
 struct CrossAttnArgs {
   const void* q;      // [batch * q_rows_per_batch, q_row_stride] 16-bit; queries are columns [head][head_dim] of each row

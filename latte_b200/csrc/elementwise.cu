@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const float* __
 // ---------------------------------------------------------------------------------- patch_embed
 constexpr int PE_TOK = 16;
 
-// K = C*p*p is a template parameter (16 for the 4-channel, patch-2 latents every Latte config uses).  A thread owns FOUR
+// K = C*p*p is a template parameter, 4 to 32 (16 for the 4-channel, patch-2 latents; wider K: patch_embed_wide_kernel).  A thread owns FOUR
 // consecutive output channels: their 4 x K weights live in registers, and for each of the block's PE_TOK tokens it does
 // 4 x K FMAs, one 16-byte read of pos_embed and ONE 16-byte store of the fp32 residual stream (the only real traffic:
 // T*D*4 bytes).  Round 1 stored 4 bytes per thread per token: 42 us for 37.7 MB; this form issues a quarter of the
@@ -267,6 +267,76 @@ __global__ void __launch_bounds__(320) patch_embed_kernel(const float* __restric
         a0 = fmaf(v, wk[0][k], a0); a1 = fmaf(v, wk[1][k], a1); a2 = fmaf(v, wk[2][k], a2); a3 = fmaf(v, wk[3][k], a3);
       }
       reinterpret_cast<float4*>(out + static_cast<size_t>(tok) * dim)[d4] = make_float4(a0 + pe.x, a1 + pe.y, a2 + pe.z, a3 + pe.w);
+    }
+  }
+}
+
+// K = 64 and 256 (patch 4 and 8 of 4-channel latents): 4 x K weights no longer fit in registers (1,024 floats at K = 256), so
+// the thread keeps the 4 x PE_TOK accumulators instead and streams K through them PE_KC columns at a time: a chunk's 4 x PE_KC
+// weights are loaded once and applied to all PE_TOK tokens of the shared `in` tile.  Each accumulator starts at the bias and
+// takes its K products in k order, as in patch_embed_kernel, all in fp32.
+constexpr int PE_KC = 16;
+
+template <int K>
+__global__ void __launch_bounds__(320) patch_embed_wide_kernel(const float* __restrict__ x, int x_batch_mod,
+                                                               const float* __restrict__ w, const float* __restrict__ bias,
+                                                               const float* __restrict__ pos, float* __restrict__ out,
+                                                               int total_tokens, int frames, int chans, int size, int patch,
+                                                               int dim, long long sb, long long sf, long long sc) {
+  static_assert(K % PE_KC == 0, "K must be a multiple of the chunk");
+  __shared__ float in[PE_TOK][K];
+  const int grid = size / patch;
+  const int N = grid * grid;
+  const int tok0 = blockIdx.x * PE_TOK;
+  for (int i = threadIdx.x; i < PE_TOK * K; i += blockDim.x) {
+    const int tl = i / K, k = i % K;
+    const int tok = tok0 + tl;
+    float val = 0.f;
+    if (tok < total_tokens) {
+      const int n = tok % N, bf = tok / N;
+      const int b = bf / frames, f = bf % frames;
+      const int bsrc = b % x_batch_mod;
+      const int gh = n / grid, gw = n % grid;
+      const int c = k / (patch * patch), ij = k % (patch * patch);
+      const int ii = ij / patch, jj = ij % patch;
+      val = x[bsrc * sb + f * sf + c * sc + static_cast<long long>(gh * patch + ii) * size + gw * patch + jj];
+    }
+    in[tl][k] = val;
+  }
+  __syncthreads();
+  const int nv = dim >> 2;
+  for (int d4 = threadIdx.x; d4 < nv; d4 += blockDim.x) {
+    const float4 bd = __ldg(reinterpret_cast<const float4*>(bias) + d4);
+    float acc[PE_TOK][4];
+#pragma unroll
+    for (int tl = 0; tl < PE_TOK; ++tl) { acc[tl][0] = bd.x; acc[tl][1] = bd.y; acc[tl][2] = bd.z; acc[tl][3] = bd.w; }
+#pragma unroll 1
+    for (int k0 = 0; k0 < K; k0 += PE_KC) {
+      float wk[4][PE_KC];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int k = 0; k < PE_KC; k += 4) {
+          const float4 t = __ldg(reinterpret_cast<const float4*>(w + static_cast<size_t>(d4 * 4 + r) * K + k0 + k));
+          wk[r][k] = t.x; wk[r][k + 1] = t.y; wk[r][k + 2] = t.z; wk[r][k + 3] = t.w;
+        }
+#pragma unroll
+      for (int tl = 0; tl < PE_TOK; ++tl)
+#pragma unroll
+        for (int k = 0; k < PE_KC; ++k) {
+          const float v = in[tl][k0 + k];
+#pragma unroll
+          for (int r = 0; r < 4; ++r) acc[tl][r] = fmaf(v, wk[r][k], acc[tl][r]);
+        }
+    }
+#pragma unroll
+    for (int tl = 0; tl < PE_TOK; ++tl) {
+      const int tok = tok0 + tl;
+      if (tok < total_tokens) {
+        const float4 pe = __ldg(reinterpret_cast<const float4*>(pos + static_cast<size_t>(tok % N) * dim) + d4);
+        reinterpret_cast<float4*>(out + static_cast<size_t>(tok) * dim)[d4] =
+            make_float4(acc[tl][0] + pe.x, acc[tl][1] + pe.y, acc[tl][2] + pe.z, acc[tl][3] + pe.w);
+      }
     }
   }
 }
@@ -693,8 +763,8 @@ int launch_patch_embed(const float* x, int x_batch_mod, const float* w, const fl
                        int batch, int frames, int chans, int size, int patch, int dim, int channels_first, cudaStream_t stream) {
   const int K = chans * patch * patch;
   B200_REQUIRE(size % patch == 0, B200_ERR_SHAPE, "patch_embed: size %d not divisible by patch %d", size, patch);
-  B200_REQUIRE(K == 4 || K == 8 || K == 16 || K == 32 || K == 64, B200_ERR_UNSUPPORTED,
-               "patch_embed: C*p*p = %d unsupported (4, 8, 16, 32, 64)", K);
+  B200_REQUIRE(K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 256, B200_ERR_UNSUPPORTED,
+               "patch_embed: C*p*p = %d unsupported (4, 8, 16, 32, 64, 256)", K);
   const int grid = size / patch;
   const int total = batch * frames * grid * grid;
   const int blocks = (total + PE_TOK - 1) / PE_TOK;
@@ -703,13 +773,14 @@ int launch_patch_embed(const float* x, int x_batch_mod, const float* w, const fl
   const long long sb = plane * chans * frames;
   const long long sf = channels_first ? plane : plane * chans;
   const long long sc = channels_first ? plane * frames : plane;
-#define B200_PE(KK) patch_embed_kernel<KK><<<blocks, 320, 0, stream>>>(x, x_batch_mod, w, b, pos, out, total, frames, chans, size, patch, dim, sb, sf, sc)
+#define B200_PE(KERNEL, KK) KERNEL<KK><<<blocks, 320, 0, stream>>>(x, x_batch_mod, w, b, pos, out, total, frames, chans, size, patch, dim, sb, sf, sc)
   switch (K) {
-    case 4: B200_PE(4); break;
-    case 8: B200_PE(8); break;
-    case 16: B200_PE(16); break;
-    case 32: B200_PE(32); break;
-    default: B200_PE(64); break;
+    case 4: B200_PE(patch_embed_kernel, 4); break;
+    case 8: B200_PE(patch_embed_kernel, 8); break;
+    case 16: B200_PE(patch_embed_kernel, 16); break;
+    case 32: B200_PE(patch_embed_kernel, 32); break;
+    case 64: B200_PE(patch_embed_wide_kernel, 64); break;
+    default: B200_PE(patch_embed_wide_kernel, 256); break;
   }
 #undef B200_PE
   B200_CHECK_CUDA(cudaGetLastError());

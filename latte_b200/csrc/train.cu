@@ -1488,6 +1488,15 @@ int launch_attention_bwd(const void* qkv, const void* o, const void* d_o, void* 
     if (bf16) return attn_bwd_two_pass<true, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
     return attn_bwd_two_pass<false, 64, true>(q, oo, g, dq, lse, delta, nseq, frames, heads, stream, tokens);
   }
+  if (!temporal && tokens <= 16) {
+    // Spatial sequences of N <= 16 tokens (patch 8 at 256^2, small grids): N consecutive rows per (b, f) are exactly the
+    // temporal kernel's input with batch' = batch * frames, frames' = N and tokens' = 1 -- one sequence of <= 16 rows per warp
+    // at row stride 1.
+    batch *= frames;
+    frames = tokens;
+    tokens = 1;
+    temporal = 1;
+  }
   if (temporal) {                                 // 1..16 frames: one warp per (b, n, head) on tensor cores
     B200_REQUIRE(head_dim == 64 || head_dim == 72, B200_ERR_UNSUPPORTED,
                  "attention_bwd: temporal sequences of 1..16 frames need head_dim 64 or 72 (got %d frames, head_dim %d)", frames, head_dim);

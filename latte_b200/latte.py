@@ -287,7 +287,7 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             in_channels=self.in_channels, out_channels=self.out_channels, input_size=self.input_size,
             frames=self.num_frames,
             num_embed=(self.y_embedder.embedding_table.weight.shape[0] if self.extras == 2 else 0),
-            dtype=_lib.BF16 if od == torch.bfloat16 else _lib.FP16)
+            dtype=_lib.BF16 if od == torch.bfloat16 else _lib.FP16, wide_patch=1)
         self._packed = (shape, w, T, od)  # T keeps the device tensors alive
         self._packed_key = key
         return self._packed

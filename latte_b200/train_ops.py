@@ -48,10 +48,15 @@ class NativeOps:
 
     def wgrad(self, dW32, dy, x):
         """dW32 [n_out, n_in] += dy [rows, n_out]^T @ x [rows, n_in]: the GEMM reads both activations untransposed (MN-major
-        operand mode); shapes it does not take (n_in not a multiple of 128) go through explicit 16-bit transposes."""
+        operand mode); shapes it does not take (n_in not a multiple of 128) go through explicit 16-bit transposes.  rows is
+        the GEMM's K: a count that is not a multiple of 64 (patch 4 and 8 give 16 or 4 tokens per frame) gets zero rows."""
         self._cuda(dW32, dy, x)
         rows, n_out = dy.shape
         n_in = x.shape[1]
+        if rows % 64:
+            pad = 64 - rows % 64
+            dy, x = torch.cat((dy, dy.new_zeros(pad, n_out))), torch.cat((x, x.new_zeros(pad, n_in)))
+            rows += pad
         if n_in % 128 == 0 and n_out % 8 == 0 and rows % 64 == 0:
             assert dy.is_contiguous() and x.is_contiguous() and dW32.is_contiguous() and dW32.dtype == torch.float32
             with torch.cuda.device(dy.device):

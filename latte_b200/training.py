@@ -79,6 +79,11 @@ def _patch_rows(x, p):
     return xx.reshape(B * Fr * (H // p) * (Wd // p), C * p * p)
 
 
+def _pad64(n):
+    """n rounded up to the GEMM's 64-element k-block."""
+    return (n + 63) // 64 * 64
+
+
 def _f32(ts):
     """fp32 copy of parameters stacked by rows (the parameter itself when it is one fp32 tensor)."""
     return ts[0].detach().float().contiguous() if len(ts) == 1 else torch.cat([t.detach().float() for t in ts])
@@ -140,7 +145,8 @@ class _EngineBase:
         [N][K], dgrad reads the same memory as an MN-major operand.  The 16-bit buffers persist on the model between steps
         (`model._train_operands`); a step refreshes all of them with one multi-tensor cast launch.  Stacked operands (the adaLN
         weights of all Latte blocks, q|k|v, every LatteT2V layer's k|v) are one buffer whose row slices are the parameters'
-        copies.  Patch-embed / output-projection operands are zero-padded to the GEMM's 64-element k-block (K = 16 and 32)."""
+        copies.  Patch-embed / output-projection operands are zero-padded to a multiple of the GEMM's 64-element k-block
+        (`_pad64`: K = C*p*p = 16 -> 64, 64, 256; the head's p*p*C_out rows 32 -> 64, 64, 128, 256, 512)."""
         m, ops, D = self.m, self.ops, self.D
         dev = self.final_linear.weight.device
         cache = getattr(m, "_train_operands", None)
@@ -164,14 +170,14 @@ class _EngineBase:
         W = {k: (cache["w"][k], _f32(bs)) for k, _, bs in self.table}
         pw = self.patch_conv.weight.detach().reshape(D, -1).float()
         self.kp = pw.shape[1]
-        pad = torch.zeros(D, 64, dtype=torch.float32, device=dev)
+        pad = torch.zeros(D, _pad64(self.kp), dtype=torch.float32, device=dev)
         pad[:, : self.kp] = pw
         W["patch"] = (ops.cast(pad), self.patch_conv.bias.detach().float().contiguous())
         fw = self.final_linear.weight.detach().float()              # [p*p*Cout, D]
         self.nf = fw.shape[0]
-        padk = torch.zeros(64, D, dtype=torch.float32, device=dev)
+        padk = torch.zeros(_pad64(self.nf), D, dtype=torch.float32, device=dev)
         padk[: self.nf] = fw
-        W["final_wk"] = ops.cast(padk)                              # rows [0, nf) = the weight (forward), all 64 rows = dgrad operand
+        W["final_wk"] = ops.cast(padk)                              # rows [0, nf) = the weight (forward), all rows = dgrad operand
         W["final"] = (W["final_wk"][: self.nf], self.final_linear.bias.detach().float().contiguous())
         self.w = W
 
@@ -343,7 +349,7 @@ class _EngineBase:
         S = {"B": B, "c": c, "sc": sc, "mod": mod, "blocks": []}
         self._context_forward(S, save)
 
-        xp = torch.zeros(T, 64, dtype=torch.float32, device=dev)
+        xp = torch.zeros(T, _pad64(self.kp), dtype=torch.float32, device=dev)
         xp[:, : self.kp] = self._patchify(x.float())
         xp = ops.to_operand(xp)
         xs = self.pos_table.detach().float().reshape(1, N, D).expand(B * (self.Fr + self.images), N, D).reshape(T, D).contiguous()
@@ -384,7 +390,7 @@ class _EngineBase:
         dtok = self._patchify_out(dout.float())                                         # (T, nf) fp32
         ops.colsum(dtok, bgrad["final"])
         G["final"] = self._wgrad(ops.to_operand(dtok), S["hf"])
-        dtp = torch.zeros(T, 64, dtype=torch.float32, device=dev)
+        dtp = torch.zeros(T, _pad64(self.nf), dtype=torch.float32, device=dev)
         dtp[:, : self.nf] = dtok
         dhf = ops.dgrad(ops.to_operand(dtp), W["final_wk"])
         dx = torch.zeros(T, D, dtype=torch.float32, device=dev)

@@ -31,11 +31,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-from .training import _EngineBase
-
-
-def _pad64(n):
-    return (n + 63) // 64 * 64
+from .training import _EngineBase, _pad64
 
 
 class T2VTrainEngine(_EngineBase):
