@@ -54,7 +54,10 @@ def _run(op, srcs, dsts, a=0.0, b=0.0, scalar=None, accum=None):
 
 
 def get_grad_norm(parameters, norm_type: float = 2.0) -> torch.Tensor:
-    """utils.py:45-70: the 2-norm of all gradients viewed as one vector (accumulated in float64 on the device)."""
+    """utils.py:45-70: the 2-norm of all gradients viewed as one vector.  Each thread of the multi-tensor kernel sums its
+    squares in fp32 and each warp sums its threads in fp32; one thread per block adds the block's 8 warp sums in float64 and
+    adds that to the total with one float64 atomic.  The relative error therefore grows linearly with the elements per
+    thread (tests/test_gpu_train_gemm_fp64.py)."""
     if isinstance(parameters, torch.Tensor):
         parameters = [parameters]
     grads = [p.grad.detach() for p in parameters if p.grad is not None]
