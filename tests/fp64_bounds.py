@@ -1,5 +1,5 @@
 """Element-by-element error bounds against fp64 references, shared by the fp64 kernel tests (test_gpu_train_ops_fp64.py,
-test_gpu_forward_ops_fp64.py).  Each output element must satisfy
+test_gpu_forward_ops_fp64.py, test_gpu_t5_fp64.py, test_gpu_t2v_glue_fp64.py).  Each output element must satisfy
 
     |got - ref| <= A * u_out * |ref| + B * u_op * mag + floor
 
@@ -14,8 +14,11 @@ U16 = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}
 U32 = 2.0 ** -24
 SUB = {torch.float16: 2.0 ** -24, torch.bfloat16: 0.0}     # subnormal spacing of the 16-bit type (bf16: none that matters)
 TANH_U = 2.0 ** -11                                          # tanh.approx.f32 relative error
+EX2_U = 2.0 ** -22                                           # ex2.approx.f32 relative error
 LOG2E = 1.4426950408889634
+GELU_K0, GELU_K1 = 0.7978845608028654, 0.044715
 A, B, F = 2.0, 4.0, 3.0
+ACC = 1.0        # forward fp32 tensor-core accumulation: u_op = ACC * sqrt(K) * 2^-24 (measured in test_gpu_forward_ops_fp64.py)
 
 
 def dtn(dt):
@@ -65,6 +68,55 @@ def sqfloor(x, y, s, lhs_t=False):
     if lhs_t:
         xm = xm.transpose(-1, -2)
     return F * (xm @ (y * y)).sqrt()
+
+
+def gelu_fwd_terms(pre, uacc, mag):
+    """fp64 gelu_tanh(pre) of a GEMM pre-activation and its bound term B * (...) without the output rounding: |gelu'(pre)|
+    uacc mag for the accumulation, tanh.approx.f32 (relative 2^-11 of t = tanh(u)) times 0.5 |pre|, and four fp32
+    roundings of u = k0 (x + k1 x^3) times 0.5 |pre| (1 - t^2) |u|."""
+    u = GELU_K0 * (pre + GELU_K1 * pre ** 3)
+    t = torch.tanh(u)
+    ref = 0.5 * pre * (1 + t)
+    dg = (0.5 * (1 + t) + 0.5 * pre * (1 - t * t) * GELU_K0 * (1 + 3 * GELU_K1 * pre ** 2)).abs()
+    return ref, B * (dg * uacc * mag + 0.5 * pre.abs() * (TANH_U * t.abs() + 4 * U32 * u.abs() * (1 - t * t)))
+
+
+def silu_err(x, e_in):
+    """First-order error of silu(x) = x / (1 + __expf(-x)) given an input error e_in: |silu'(x)| e_in, the __expf error
+    (2 + 1.173 |x| ulp of fp32) and the rounding of 1 + e and of the division."""
+    sg = torch.sigmoid(x)
+    d = (sg * (1 + x * (1 - sg))).abs()
+    return d * e_in + U32 * (2 * (2 + 1.173 * x.abs()) + 2) * (x * sg).abs()
+
+
+def softmax_fwd_terms(q, k, v, bias, dt, scale=None):
+    """fp64 softmax(q k^T scale + bias) v (q [.., Sq, hd], k / v [.., Sk, hd]; scale None = hd^-1/2; bias None or an additive
+    fp32 score bias broadcast to [.., Sq, Sk]) and its bound terms B * u_op * mag + floor, with u_op per query row =
+    2^-11 / 2^-8 (P rounded to 16 bits before the PV product) + 2 * 2^-24 * log2(e) * max|s| (the fp32 exp2 argument) +
+    2^-22 (ex2.approx.f32) + ACC * sqrt(hd) * 2^-24 * max_j |q| |k_j| * scale (the fp32 QK^T) + sqrt(Sk) * 2^-24 (the fp32
+    PV and l sums), and mag = sum_j p_j |v_j|.  max|s| is taken over the keys with p_j > 0 only: an error in the exp2 argument
+    of key j moves p_j by a relative 2^-24 |s_j| ln 2, nothing for a key whose probability is 0 in fp64 and in fp32 (a -1e30
+    padding key: ex2 of about -1.4e30; a -10000 key beside an unmasked one: ex2 of about -14000).  Such keys inside max|s|
+    would make the bound ~1e23 for the -1e30 padding and accept anything.  fp16 floor: 2^-24 plus
+    F * p_max * sqrt(sum_j (min(2^-24, P_j) |v_j|)^2), P_j = p_j / p_max the unnormalised probability the kernel rounds.
+    Returns (out, term, p)."""
+    hd, S = q.shape[-1], k.shape[-2]
+    sc = hd ** -0.5 if scale is None else scale
+    s = q @ k.transpose(-1, -2) * sc
+    if bias is not None:
+        s = s + bias
+    p = torch.softmax(s, -1)
+    out = p @ v
+    qk = (q.abs() @ k.abs().transpose(-1, -2)) * sc
+    smax = torch.where(p > 0, s.abs(), torch.zeros_like(s)).amax(-1, keepdim=True)
+    u_row = (U16[dt] + EX2_U + 2 * U32 * LOG2E * smax + ACC * math.sqrt(hd) * U32 * qk.amax(-1, keepdim=True)
+             + math.sqrt(S) * U32)
+    del s, qk
+    term = B * u_row * (p @ v.abs())
+    if SUB[dt]:
+        pmax = p.amax(-1, keepdim=True)
+        term += sqfloor(p / pmax, v, SUB[dt]) * pmax + SUB[dt]
+    return out, term, p
 
 
 # ------------------------------------------------------------------------------------------------ attention layouts

@@ -31,7 +31,8 @@ kernel reads.  Every output element must satisfy (tests/fp64_bounds.py, A = 2, B
         most 4 roundings of values below mag: 4 * 2^-24 <= sqrt(K) * 2^-24 for every K >= 16.
   * Attention (spatial, temporal, cross).  mag = sum_j p_j |v_j| (p the softmax); u_op per query row = 2^-11 / 2^-8 (P
     is rounded to 16 bits before the PV product; its sum l stays fp32) + 2 * 2^-24 * log2(e) * max|s| (the fp32 exp2
-    argument s * scale * log2(e), natural-log scores s, +-30 logits, -10000 key biases) + 2^-22 (ex2.approx.f32) +
+    argument s * scale * log2(e), natural-log scores s, +-30 logits, -10000 key biases; the max runs over the keys with
+    nonzero probability, tests/fp64_bounds.softmax_fwd_terms) + 2^-22 (ex2.approx.f32) +
     ACC * sqrt(hd) * 2^-24 * max_j |q| |k_j| * scale (the fp32 QK^T) + sqrt(S) * 2^-24 (the fp32 PV and l sums).  fp16
     floor: 2^-24 plus F * p_max * sqrt(sum_j (min(2^-24, P_j) |v_j|)^2) with P_j = p_j / p_max the unnormalised
     probability the kernel rounds (its subnormals are off by up to half a spacing each, independently).
@@ -61,14 +62,10 @@ import pytest
 import torch
 import torch.nn.functional as Fn
 
-from fp64_bounds import A, B, DTS, LOG2E, SUB, TANH_U, U16, U32, Checker, report_worst, sqfloor  # noqa: E402
-from fp64_bounds import edge_rows, to_rows, to_seq  # noqa: E402
+from fp64_bounds import A, ACC, B, DTS, GELU_K0, GELU_K1, SUB, U16, U32, Checker, report_worst, sqfloor  # noqa: E402
+from fp64_bounds import edge_rows, gelu_fwd_terms, silu_err, softmax_fwd_terms, to_rows, to_seq  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-
-ACC = 1.0                     # fp32 tensor-core accumulation: u_op = ACC * sqrt(K) * 2^-24 (measured, see the docstring)
-EX2_U = 2.0 ** -22            # ex2.approx.f32 relative error
-GELU_K0, GELU_K1 = 0.7978845608028654, 0.044715
 
 _WORST = {}
 _ACC_TABLE = {}
@@ -179,12 +176,9 @@ def test_linear(dev, dt, M, shape):
     # bias epilogue (qkv)
     bnd_bias = A * U16[dt] * pre.abs() + B * uacc * mag + sub
     # GELU epilogue (fc1)
-    u = GELU_K0 * (pre + GELU_K1 * pre ** 3)
-    t = torch.tanh(u)
-    ref_gelu = 0.5 * pre * (1 + t)
-    dg = (0.5 * (1 + t) + 0.5 * pre * (1 - t * t) * GELU_K0 * (1 + 3 * GELU_K1 * pre ** 2)).abs()
-    bnd_gelu = A * U16[dt] * ref_gelu.abs() + B * (dg * uacc * mag + 0.5 * pre.abs() * (TANH_U * t.abs() + 4 * U32 * u.abs() * (1 - t * t))) + sub
-    del u, dg
+    ref_gelu, term = gelu_fwd_terms(pre, uacc, mag)
+    bnd_gelu = A * U16[dt] * ref_gelu.abs() + term + sub
+    del term
     # gated residual (proj / fc2 / head)
     bidx = torch.arange(M, device=dev) // rpb
     g64 = gate.double()[bidx]
@@ -250,27 +244,6 @@ def test_gemm_accumulation(dev, dt):
 
 
 # ------------------------------------------------------------------------------------------------ attention
-def _softmax_fwd_terms(q, k, v, bias, dt):
-    """fp64 softmax(q k^T hd^-1/2 + bias) v (q [.., Sq, hd], k / v [.., Sk, hd]) and its bound terms B * u_op * mag + floor
-    (see the module docstring)."""
-    hd, S = q.shape[-1], k.shape[-2]
-    sc = hd ** -0.5
-    s = q @ k.transpose(-1, -2) * sc
-    if bias is not None:
-        s = s + bias
-    p = torch.softmax(s, -1)
-    out = p @ v
-    qk = (q.abs() @ k.abs().transpose(-1, -2)) * sc
-    u_row = (U16[dt] + EX2_U + 2 * U32 * LOG2E * s.abs().amax(-1, keepdim=True)
-             + ACC * math.sqrt(hd) * U32 * qk.amax(-1, keepdim=True) + math.sqrt(S) * U32)
-    del s, qk
-    term = B * u_row * (p @ v.abs())
-    if SUB[dt]:
-        pmax = p.amax(-1, keepdim=True)
-        term += sqfloor(p / pmax, v, SUB[dt]) * pmax + SUB[dt]
-    return out, term, p
-
-
 def _attention_case(dev, dt, Bb, Fr, N, H, hd, temporal):
     from latte_b200 import ops
     chk = _chk(dt)
@@ -296,7 +269,7 @@ def _attention_case(dev, dt, Bb, Fr, N, H, hd, temporal):
     for c0 in range(0, nseq, step):
         c1 = min(nseq, c0 + step)
         q, k, v = qs[c0:c1, 0], qs[c0:c1, 1], qs[c0:c1, 2]
-        ref, term, _ = _softmax_fwd_terms(q, k, v, None, dt)
+        ref, term, _ = softmax_fwd_terms(q, k, v, None, dt)
         bnd = A * U16[dt] * ref.abs() + term
         chk.add(f"attention {kind}", tag, got[c0:c1], ref, bnd, where(c0))
         if c0 == 0 and S > 1:       # a kernel that drops the last key of every sequence
@@ -364,14 +337,14 @@ def test_cross_attention(dev, dt, case):
     k4, v4 = kv5[:, :, 0].transpose(1, 2), kv5[:, :, 1].transpose(1, 2)
     for n0 in range(Bn):
         b4 = bias[n0:n0 + 1, None, None, :L].double() if bias is not None else None
-        ref, term, _ = _softmax_fwd_terms(q4[n0:n0 + 1], k4[n0:n0 + 1], v4[n0:n0 + 1], b4, dt)
+        ref, term, _ = softmax_fwd_terms(q4[n0:n0 + 1], k4[n0:n0 + 1], v4[n0:n0 + 1], b4, dt)
         bnd = A * U16[dt] * ref.abs() + term
 
         def where(i, n0=n0):
             return f"sample {n0}, head {i[1]}, query {i[2]}, dim {i[3]}"
         chk.add(f"cross_attention {'key_bias' if bias is not None else 'no bias'}", f"{case}", got[n0:n0 + 1], ref, bnd, where)
         if bias is not None and n0 == 0:
-            free, _, _ = _softmax_fwd_terms(q4[:1], k4[:1], v4[:1], None, dt)
+            free, _, _ = softmax_fwd_terms(q4[:1], k4[:1], v4[:1], None, dt)
             _rejects(dt, "cross_attention: key_bias ignored", (got[:1].double() + free - ref).to(dt), ref, bnd)
     chk.done()
 
@@ -445,14 +418,6 @@ def _latte(dev, dt, D, heads, extras, learn_sigma, depth=2, frames=4, input_size
     return cfg, {k: v.to(dev) for k, v in sd.items()}, net
 
 
-def _silu_err(x, e_in):
-    """First-order error of silu(x) = x / (1 + __expf(-x)) given an input error e_in: |silu'(x)| e_in, the __expf error
-    (2 + 1.173 |x| ulp of fp32) and the rounding of 1 + e and of the division."""
-    sg = torch.sigmoid(x)
-    d = (sg * (1 + x * (1 - sg))).abs()
-    return d * e_in + U32 * (2 * (2 + 1.173 * x.abs()) + 2) * (x * sg).abs()
-
-
 @pytest.mark.parametrize("dt", DTS)
 @pytest.mark.parametrize("D,heads", [(384, 6), (1152, 16)])
 @pytest.mark.parametrize("extras", [1, 2])
@@ -486,11 +451,11 @@ def test_conditioning(dev, dt, D, heads, extras):
     h1 = tf @ W0.t() + b0
     e = e @ W0.abs().t() + U32 * math.sqrt(256) * (tf.abs() @ W0.abs().t() + b0.abs())
     s1 = Fn.silu(h1)
-    e = _silu_err(h1, e)
+    e = silu_err(h1, e)
     lab = O.y_embedder(sd64, yy, torch.float64).abs() if extras == 2 else 0
     e = e @ W2.abs().t() + U32 * math.sqrt(D) * (s1.abs() @ W2.abs().t() + b2.abs() + lab)
     sc = Fn.silu(c)
-    e = _silu_err(c, e)
+    e = silu_err(c, e)
     e = e @ w16.abs().t() + U32 * math.sqrt(D) * (sc.abs() @ w16.abs().t() + ab.abs())
     bnd = A * U32 * ref.abs() + B * e
     chk.add("conditioning adaLN rows", f"D={D} extras={extras}", got, ref, bnd,
