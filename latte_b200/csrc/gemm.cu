@@ -50,7 +50,9 @@ constexpr int kEpiBufBytes = 64 * 128;
 
 template <int BN, int EPI>
 struct Cfg {
+  static constexpr int BLOCK_N = BN;
   static constexpr bool RESID = EPI == B200_EPI_GATE_RESIDUAL;
+  static constexpr bool TWO_OUT = EPI == B200_EPI_BIAS_GELU_BOTH;   // out16 and out16b
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;                       // the whole W tile (both CTAs' halves)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
@@ -170,6 +172,183 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return fmaf(hx, t, hx);
 }
 
+// ----------------------------------------------------------------------------- the pieces both GEMM kernels are made of
+// gemm_kernel and fp8_linear_kernel share the structure described at the top of this file through the code below: the
+// prologue, the pair-tile geometry, the TMA producer loop, the consumers' stage bookkeeping and the 16-bit output
+// epilogue.  What each kernel loads per stage, how it multiplies a k-block and how it computes an output value are its own.
+
+// One CTA's operand pipeline in the Cfg layout: STAGES slots, each with a "full" and an "empty" barrier.
+template <class C>
+struct Pipeline {
+  uint8_t* smem;     // dynamic shared memory, 1 KiB aligned: the 128B swizzle's period
+  uint64_t* full;    // this CTA's expect_tx arrival; the bytes of A and of both W halves complete it
+  uint64_t* empty;   // one arrival per consumer warpgroup of BOTH CTAs (each W half lands in both)
+  __device__ __forceinline__ uint8_t* slot(int stage) const { return smem + stage * C::STAGE_BYTES; }
+};
+
+// Thread 0 prefetches the tensor maps and initialises the barriers.  The cluster barrier has both CTAs' barriers
+// initialised before any multicast / remote arrival can target them; then the next kernel may begin its prologue as SMs
+// drain (PDL).
+template <class C, class... Maps>
+__device__ __forceinline__ Pipeline<C> gemm_prologue(const Maps*... maps) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
+  const Pipeline<C> pl{smem, bars, bars + C::STAGES};
+  if (threadIdx.x == 0) {
+    (tma_prefetch_desc(maps), ...);
+    for (int i = 0; i < C::STAGES; ++i) {
+      mbar_init(&pl.full[i], 1);
+      mbar_init(&pl.empty[i], 4);
+    }
+    fence_mbar_init();
+  }
+  cluster_sync_all();
+  pdl_launch_dependents();
+  return pl;
+}
+
+// Pair-tile geometry: cluster k owns pair-tiles k, k + #clusters, ... (TileSched); a pair-tile is two M-adjacent 128-row
+// tiles of one BN-wide column, and this CTA takes row-tile m_blk = 2 * pair_m + rank (it may lie past M: zero-filled
+// loads, clipped stores).  Each CTA fetches half of the W tile, rows w_row0 .. w_row0 + BN/2, and multicasts it to both.
+template <int BN>
+struct PairTiles {
+  const GemmDev& p;
+  uint32_t rank;
+  int num_tiles, my_pair, num_pairs;
+  __device__ __forceinline__ explicit PairTiles(const GemmDev& p_)
+      : p(p_), rank(cluster_ctarank()), num_tiles((p_.num_m + 1) / 2 * p_.num_n), my_pair(blockIdx.x >> 1),
+        num_pairs(gridDim.x >> 1) {}
+  __device__ __forceinline__ TileSched sched(int num_kb, bool streamk) const {
+    return TileSched(my_pair, num_pairs, num_tiles, num_kb, streamk);
+  }
+  __device__ __forceinline__ int m_blk(int tile) const { return 2 * (tile / p.num_n) + static_cast<int>(rank); }
+  __device__ __forceinline__ int n0(int tile) const { return (tile % p.num_n) * BN; }
+  __device__ __forceinline__ int w_row0(int tile) const { return n0(tile) + static_cast<int>(rank) * (BN / 2); }
+};
+
+// The TMA producer: warpgroup 0 hands its registers to the consumers, and one thread walks this CTA's k-block sequence.
+// Load q goes to slot q % STAGES; it is issued as soon as the slot's previous contents (load q - STAGES) have been released
+// by both consumer warpgroups of both CTAs, so all STAGES slots stay in flight, across tile boundaries and through the
+// consumers' epilogues.  The producer waits on nothing but `empty`.  load(slot, bar, m_blk, w_row0, kb) issues k-block
+// kb's TMA loads into the slot: this CTA's A tile and its W half, multicast; together they complete STAGE_BYTES on `bar`.
+template <class C, class Load>
+__device__ __forceinline__ void produce(const Pipeline<C>& pl, const PairTiles<C::BLOCK_N>& pt, int num_kb, bool streamk,
+                                        Load load) {
+  setmaxnreg_dec<kProducerRegs>();
+  if (threadIdx.x == 0) {
+    pdl_wait();                             // operands: visible from here
+    TileSched sched = pt.sched(num_kb, streamk);
+    int stage = 0;
+    uint32_t phase = 0;
+    int tile, kb0, kb1;
+    while (sched.next(tile, kb0, kb1)) {
+      const int m_blk = pt.m_blk(tile), w_row0 = pt.w_row0(tile);
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&pl.empty[stage], phase ^ 1);  // both CTAs' consumer warpgroups are done with the slot
+        mbar_arrive_expect_tx(&pl.full[stage], C::STAGE_BYTES);
+        load(pl.slot(stage), &pl.full[stage], m_blk, w_row0, kb);
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  }
+  __syncwarp();                             // warp 0 reconverges before the cluster barrier
+}
+
+// A consumer thread: warpgroups 1-2, one 64-row half of the tile each, after raising their register budget.
+// Accumulator fragment: thread (w4, g, cq) holds rows lr0 = 16*w4 + g and lr0 + 8 of its warpgroup's 64, columns
+// 8j + 2cq + {0,1}: acc[4j + 2h + {0,1}] for row lr0 + 8h.
+// Stages: wait() returns the next one's shared address once it is full.  After wgmma_wait<1>, release_prev() frees the
+// slot of the k-block before in both CTAs (the peer's next multicast writes into it); after the tile's wgmma_wait<0>,
+// release_last() frees the tile's last slot.
+// Staging buffers: warpgroup wg owns epi buffers 2 wg and 2 wg + 1; chunk i of its output uses buffer i % 2 (ep counts).
+template <class C>
+struct Consumer {
+  Pipeline<C> pl;
+  int wg, te, lane, w4, g, cq, lr0;
+  uint32_t empty_peer;
+  uint8_t* epi;
+  int stage = 0, prev = -1, ep = 0;
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ Consumer(const Pipeline<C>& pl_, uint32_t rank, int wg_) : pl(pl_), wg(wg_) {
+    setmaxnreg_inc<kConsumerRegs>();
+    pdl_wait();                               // bias / scales / side inputs / residual stream: visible from here
+    lane = threadIdx.x & 31;
+    te = threadIdx.x & 127;
+    w4 = te >> 5, g = lane >> 2, cq = lane & 3;
+    lr0 = w4 * 16 + g;
+    empty_peer = mapa_u32(&pl.empty[0], rank ^ 1u);
+    epi = pl.smem + C::EPI_OFF;
+  }
+  __device__ __forceinline__ uint32_t wait() {
+    mbar_wait(&pl.full[stage], phase);
+    return smem_u32(pl.slot(stage));
+  }
+  __device__ __forceinline__ void release_prev() {
+    if (prev >= 0 && te == 0) {
+      mbar_arrive(&pl.empty[prev]);
+      mbar_arrive_cluster(empty_peer + prev * 8);
+    }
+    prev = stage;
+    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+  }
+  __device__ __forceinline__ void release_last() {
+    if (te == 0) {
+      mbar_arrive(&pl.empty[prev]);
+      mbar_arrive_cluster(empty_peer + prev * 8);
+    }
+    prev = -1;
+  }
+
+  // The 16-bit output epilogue: out16 (and out16b with TWO_OUT, in both buffers per chunk) in 64-column chunks.
+  // vals(j, col, col_ok, v, vb) packs the two 16-bit values of column group j (matrix columns col, col + 1) for rows
+  // lr0 and lr0 + 8 into v[0], v[1] (and vb[0], vb[1]), each rounded exactly as a direct store would round it; stmatrix
+  // writes them into the swizzled buffer: an 8x8 matrix is 8 rows x one 16-byte unit, the rows in 8 different bank groups.
+  template <class Vals>
+  __device__ __forceinline__ void store16(const CUtensorMap* tmC, const CUtensorMap* tmC2, int m0w, int n0, int N, Vals vals) {
+    constexpr bool TWO = C::TWO_OUT;
+    const int mi = lane >> 3;                               // the matrix whose row this lane addresses
+    const int lrow = w4 * 16 + (lane & 7) + 8 * (mi & 1);
+#pragma unroll
+    for (int c = 0; c < C::BLOCK_N / 64; ++c) {
+      if (n0 + 64 * c >= N) break;           // N % 32 == 0: the last chunk may be half inside N; TMA clips the rest
+      uint8_t* buf = epi + (2 * wg + (TWO ? 0 : (ep & 1))) * kEpiBufBytes;
+      const uint32_t row_addr = smem_u32(buf) + lrow * 128;
+#pragma unroll
+      for (int jp = 0; jp < 4; ++jp) {       // column groups j = 8c + 2jp + q, q = 0, 1: matrix 2q + h holds rows lr0 + 8h
+        uint32_t v[4], vb[4];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int j = 8 * c + 2 * jp + q, col = n0 + 8 * j + 2 * cq;
+          vals(j, col, col < N, v + 2 * q, vb + 2 * q);
+        }
+        // this lane's row holds column group 2jp + (mi >> 1) in 16-byte unit (2jp + (mi >> 1)) ^ (lrow % 8)
+        const uint32_t unit = ((2 * jp + (mi >> 1)) ^ (lane & 7)) << 4;
+        stmatrix_x4(row_addr + unit, v[0], v[1], v[2], v[3]);
+        if constexpr (TWO) stmatrix_x4(row_addr + kEpiBufBytes + unit, vb[0], vb[1], vb[2], vb[3]);
+      }
+      fence_proxy_async_smem();              // the writes above -> visible to TMA
+      epi_bar(wg);
+      if (te == 0) {
+        tma_store_2d(tmC, buf, n0 + 64 * c, m0w);
+        if constexpr (TWO) tma_store_2d(tmC2, buf + kEpiBufBytes, n0 + 64 * c, m0w);
+        tma_store_commit();
+        // TWO rewrites both buffers every chunk; otherwise the previous chunk has been read out of the other buffer ...
+        if constexpr (TWO) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
+      }
+      epi_bar(wg);                           // ... which may now be rewritten
+      ++ep;
+    }
+  }
+
+  // every store / reduce-add of this warpgroup has been performed before the CTA retires, so the writes are complete with
+  // the grid, as a PDL-launched successor's griddepcontrol.wait expects
+  __device__ __forceinline__ void finish() const {
+    if (te == 0) tma_store_wait_all<0>();
+  }
+};
+
 // MN: operand layout.  Bit 0: A is stored [K, M]; bit 1: W is stored [K, N] (the contraction dimension is the ROW index):
 // such an operand is fetched as 64-wide MN blocks x 64 k-rows and multiplied through an MN-major wgmma descriptor.
 // wgrad uses 3 (dW = dY^T X), dgrad 2 (dX = dY W with W in its [out, in] layout), everything else 0.  A compile-time
@@ -183,138 +362,67 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   using C = Cfg<BN, EPI>;
   constexpr int TA = MN & 1, TB = MN >> 1;
   static_assert(MN == 0 || MN == 2 || MN == 3, "operand layouts: 0 forward, 2 dgrad, 3 wgrad");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + C::STAGES;
-
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
-    if constexpr (EPI == B200_EPI_BIAS_GELU_BOTH) tma_prefetch_desc(&tmC2);
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full[i], 1);    // this CTA's expect_tx arrival; the bytes of both W halves and of A complete it
-      mbar_init(&empty[i], 4);   // one arrival per consumer warpgroup of BOTH CTAs (each W half lands in both)
-    }
-    fence_mbar_init();
-  }
-  cluster_sync_all();   // barriers of both CTAs are initialised before any multicast / remote arrival can target them
-  pdl_launch_dependents();   // the next kernel may begin its prologue as SMs drain
-
-  // pair-tile schedule: cluster k owns pair-tiles k, k + #clusters, ...; a pair-tile is two M-adjacent 128-row tiles of
-  // one N column; this CTA takes row-tile 2 * pair_m + rank (it may lie past M: zero-filled loads, clipped stores)
-  const uint32_t rank = cluster_ctarank();
-  const int num_pair_m = (p.num_m + 1) / 2;
-  const int num_tiles = num_pair_m * p.num_n;
-  const int my_pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
+  const Pipeline<C> pl = C::TWO_OUT ? gemm_prologue<C>(&tmA, &tmB, &tmC, &tmC2) : gemm_prologue<C>(&tmA, &tmB, &tmC);
+  const PairTiles<BN> pt(p);
   const int num_kb = p.K / BK;
   const bool streamk = C::RESID && p.streamk != 0;
 
   if (warp < 4) {
-    // ------------------------------------------------------------------ TMA producer: warpgroup 0, one thread
-    // Load q of this CTA's k-block sequence goes to slot q % STAGES; it is issued as soon as the slot's previous contents
-    // (load q - STAGES) have been released by both consumer warpgroups of both CTAs, so all STAGES slots stay in flight,
-    // across tile boundaries and through the consumers' epilogues.  The producer waits on nothing but `empty`.
-    setmaxnreg_dec<kProducerRegs>();
-    if (threadIdx.x == 0) {
-      pdl_wait();                             // operands: visible from here
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
-      int stage = 0;
-      uint32_t phase = 0;
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
-        const int m_blk = 2 * (tile / p.num_n) + static_cast<int>(rank), n_blk = tile % p.num_n;
-        const int w_row0 = n_blk * BN + static_cast<int>(rank) * (BN / 2);   // this CTA fetches half of the W tile for both
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);  // both CTAs' consumer warpgroups are done with the slot
-          mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
-          uint8_t* sa = smem + stage * C::STAGE_BYTES;
-          if (MN == 0 && p.conv_taps > 0) {
-            // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
-            // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
-            const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
-            const int pix0 = m_blk * BM;
-            const int hw = p.conv_h * p.conv_w;
-            const int img = pix0 / hw, rem = pix0 % hw;
-            tma_load_4d(sa, &tmA, &full[stage], cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap],
-                        img + p.conv_dz[tap]);
-          } else if constexpr (TA) {
-            // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
-            // MN-major SW128 block; blocks past the live rows are zero-filled by TMA and still count their bytes
+    produce(pl, pt, num_kb, streamk, [&](uint8_t* sa, uint64_t* bar, int m_blk, int w_row0, int kb) {
+      if (MN == 0 && p.conv_taps > 0) {
+        // implicit GEMM: this k-block is channels [cb*64, +64) of filter tap `tap`; the A tile is the tile's
+        // conv_bh x conv_bw pixel patch shifted by the tap offset (borders zero-filled by TMA)
+        const int tap = kb / p.conv_cblk, cb = kb % p.conv_cblk;
+        const int pix0 = m_blk * BM;
+        const int hw = p.conv_h * p.conv_w;
+        const int img = pix0 / hw, rem = pix0 % hw;
+        tma_load_4d(sa, &tmA, bar, cb * BK, rem % p.conv_w + p.conv_dx[tap], rem / p.conv_w + p.conv_dy[tap],
+                    img + p.conv_dz[tap]);
+      } else if constexpr (TA) {
+        // operand stored [K][MN]: one box = 64 MN elements (a 128-byte swizzle row) x 64 k-rows = 8 KiB, the canonical
+        // MN-major SW128 block; blocks past the live rows are zero-filled by TMA and still count their bytes
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, &full[stage], m_blk * BM + j * 64, kb * BK);
-          } else {
-            tma_load_2d(sa, &tmA, &full[stage], kb * BK, m_blk * BM);
-          }
-          if constexpr (TB) {
-            constexpr int per_cta = BN / 128;    // 64-column blocks of W this CTA fetches
-#pragma unroll
-            for (int j = 0; j < per_cta; ++j)
-              tma_load_2d_mcast(sa + C::A_BYTES + (rank * per_cta + j) * 8192, &tmB, &full[stage], w_row0 + j * 64, kb * BK, 0x3);
-          } else {
-            tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK, w_row0, 0x3);
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
+        for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * 8192, &tmA, bar, m_blk * BM + j * 64, kb * BK);
+      } else {
+        tma_load_2d(sa, &tmA, bar, kb * BK, m_blk * BM);
       }
-    }
-    __syncwarp();                             // warp 0 reconverges before the cluster barrier
+      if constexpr (TB) {
+        constexpr int per_cta = BN / 128;    // 64-column blocks of W this CTA fetches
+#pragma unroll
+        for (int j = 0; j < per_cta; ++j)
+          tma_load_2d_mcast(sa + C::A_BYTES + (pt.rank * per_cta + j) * 8192, &tmB, bar, w_row0 + j * 64, kb * BK, 0x3);
+      } else {
+        tma_load_2d_mcast(sa + C::A_BYTES + pt.rank * (C::B_BYTES / 2), &tmB, bar, kb * BK, w_row0, 0x3);
+      }
+    });
   } else {
-    // ------------------------------------------------------------------ MMA + epilogue: warpgroups 1, 2 (64 rows each)
-    setmaxnreg_inc<kConsumerRegs>();
-    pdl_wait();                               // bias / gate / shortcut / residual stream: visible from here
-    const int wg = (warp >> 2) - 1;           // which 64-row half of the tile
-    const int te = threadIdx.x & 127;
-    const int w4 = te >> 5, g = lane >> 2, cq = lane & 3;
-    const uint32_t empty_peer = mapa_u32(&empty[0], rank ^ 1u);
-    int stage = 0;
-    uint32_t phase = 0;
+    Consumer<C> cs(pl, pt.rank, (warp >> 2) - 1);
     float acc[BN / 2];
-    uint8_t* epi = smem + C::EPI_OFF;         // this CTA's four staging buffers; warpgroup wg owns 2 wg and 2 wg + 1
-    int ep = 0;                               // chunks this warpgroup has staged so far: chunk i uses buffer i % 2
-    TileSched sched(my_pair, num_pairs, num_tiles, num_kb, streamk);
+    TileSched sched = pt.sched(num_kb, streamk);
     int tile, kb0, kb1;
     while (sched.next(tile, kb0, kb1)) {
-      const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN;
-      int prev = -1;
+      const int m0 = pt.m_blk(tile) * BM, n0 = pt.n0(tile);
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES), sb = sa + C::A_BYTES;
+        const uint32_t sa = cs.wait(), sb = sa + C::A_BYTES;
         wgmma_fence();
         // K-major: 8-row groups 1024 B apart, a k-step of 16 elements = 32 B inside the swizzle row.  MN-major: 64-wide
         // blocks 8192 B apart (leading offset), 8-k-row groups 1024 B apart, a k-step of 16 k-rows = 2048 B.
-        const uint64_t da = gmma_desc(sa + wg * 8192, TA ? 8192 : 16, 1024, GMMA_LAYOUT_SW128);
+        const uint64_t da = gmma_desc(sa + cs.wg * 8192, TA ? 8192 : 16, 1024, GMMA_LAYOUT_SW128);
         const uint64_t db = gmma_desc(sb, TB ? 8192 : 16, 1024, GMMA_LAYOUT_SW128);
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)
           WgmmaSS<BN, TA, TB, BF16>::mma(acc, gmma_desc_advance(da, k * (TA ? 2048 : 32)),
                                          gmma_desc_advance(db, k * (TB ? 2048 : 32)), (kb != kb0 || k) ? 1u : 0u);
         wgmma_commit();
-        wgmma_wait<1>();                      // the previous k-block's MMAs have read their slot: release it in both CTAs
-        if (prev >= 0 && te == 0) {
-          mbar_arrive(&empty[prev]);
-          mbar_arrive_cluster(empty_peer + prev * 8);
-        }
-        prev = stage;
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        wgmma_wait<1>();                      // the previous k-block's MMAs have read their slot
+        cs.release_prev();
       }
       wgmma_wait<0>();
       reg_fence(acc);
-      if (te == 0) {
-        mbar_arrive(&empty[prev]);
-        mbar_arrive_cluster(empty_peer + prev * 8);
-      }
+      cs.release_last();
 
-      // accumulator fragment: thread (w4, g, cq) holds rows lr0 = 16*w4 + g and lr0 + 8 of its warpgroup's 64 (which start
-      // at row m0w of the matrix), columns 8j + 2cq + {0,1}: acc[4j + 2h + {0,1}] for row lr0 + 8h
-      const int m0w = m0 + wg * 64;
-      const int lr0 = w4 * 16 + g;
+      const int m0w = m0 + cs.wg * 64;        // this warpgroup's first row
       if constexpr (C::RESID) {
         // x += gate * (acc + bias) (+ row_add) without ever loading x: the increment goes to a staging buffer in 32-column
         // chunks and TMA adds each chunk into x in L2.  Every element receives one add per GEMM -- or, for stream-K tiles,
@@ -322,7 +430,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const bool first_seg = kb0 == 0;       // bias and row_add are added once per output element
         const bool partial = kb0 > 0 || kb1 < num_kb;
         unsigned long long* flag = nullptr;
-        if (partial) flag = p.sk_flags + (static_cast<size_t>(tile - sched.full_waves * num_pairs) * 2 + rank) * 2 + wg;
+        if (partial) flag = p.sk_flags + (static_cast<size_t>(tile - sched.full_waves * pt.num_pairs) * 2 + pt.rank) * 2 + cs.wg;
         bool ordered = kb0 == 0;               // issuing thread: may this segment add into x yet?
         const float* bias = (p.bias && first_seg) ? p.bias : nullptr;
         const float* gate_row[2];
@@ -330,18 +438,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           // a row past M computes an increment from a clamped row, and the reduce-add clips it
-          const int row = m0w + lr0 + 8 * h < p.M ? m0w + lr0 + 8 * h : p.M - 1;
+          const int row = m0w + cs.lr0 + 8 * h < p.M ? m0w + cs.lr0 + 8 * h : p.M - 1;
           gate_row[h] = p.gate + static_cast<long long>(row / p.rows_per_batch) * p.gate_bs;
           add_row[h] = (p.row_add && first_seg) ? p.row_add + static_cast<size_t>((row / p.row_add_div) % p.row_add_period) * p.N : nullptr;
         }
 #pragma unroll
         for (int c = 0; c < BN / 32; ++c) {
           if (n0 + 32 * c >= p.N) break;       // N % 32 == 0: a chunk lies wholly inside N or wholly past it
-          uint8_t* buf = epi + (2 * wg + (ep & 1)) * kEpiBufBytes;
+          uint8_t* buf = cs.epi + (2 * cs.wg + (cs.ep & 1)) * kEpiBufBytes;
           const uint32_t buf_addr = smem_u32(buf);
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * c + jj, col = n0 + 8 * j + 2 * cq;
+            const int j = 4 * c + jj, col = n0 + 8 * j + 2 * cs.cq;
             const float2 b2 = bias ? __ldg(reinterpret_cast<const float2*>(bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -350,12 +458,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               const float d0 = resid_delta(acc[4 * j + 2 * h], b2.x, gt.x, ra.x, add_row[h] != nullptr);
               const float d1 = resid_delta(acc[4 * j + 2 * h + 1], b2.y, gt.y, ra.y, add_row[h] != nullptr);
               // buffer row lr0 + 8h is 128 bytes; its 16-byte units are XOR-swizzled by the row % 8 (= g), as SW128 TMA reads them
-              st_shared_f2(buf_addr + (lr0 + 8 * h) * 128 + (((2 * jj + (cq >> 1)) ^ g) << 4) + 8 * (cq & 1), d0, d1);
+              st_shared_f2(buf_addr + (cs.lr0 + 8 * h) * 128 + (((2 * jj + (cs.cq >> 1)) ^ cs.g) << 4) + 8 * (cs.cq & 1), d0, d1);
             }
           }
           fence_proxy_async_smem();            // the writes above -> visible to TMA
-          epi_bar(wg);
-          if (te == 0) {
+          epi_bar(cs.wg);
+          if (cs.te == 0) {
             if (!ordered) {
               // continuing segment: acquire the previous segment's release (it follows that segment's completed adds) ...
               flag_wait(flag, static_cast<unsigned long long>(kb0));
@@ -367,78 +475,43 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             tma_store_commit();
             tma_store_wait_read<1>();          // the previous chunk has been read out of the other buffer ...
           }
-          epi_bar(wg);                         // ... which may now be rewritten
-          ++ep;
+          epi_bar(cs.wg);                      // ... which may now be rewritten
+          ++cs.ep;
         }
-        if (partial && kb1 < num_kb && te == 0) {
+        if (partial && kb1 < num_kb && cs.te == 0) {
           tma_store_wait_all<0>();             // this segment's adds have been performed in x ...
           fence_proxy_async_global();          // ... and are ordered before the generic-proxy release:
           flag_release(flag, static_cast<unsigned long long>(kb1));   // the next segment may add
         }
       } else {
-        // 16-bit output(s) in 64-column chunks, each value rounded exactly as a direct store would round it, then stmatrix
-        // into the swizzled buffer: an 8x8 matrix is 8 rows x one 16-byte unit, the rows in 8 different bank groups
-        constexpr bool TWO = EPI == B200_EPI_BIAS_GELU_BOTH;   // out16 and out16b: both buffers per chunk
-        const int mi = lane >> 3;                               // the matrix whose row this lane addresses
-        const int lrow = w4 * 16 + (lane & 7) + 8 * (mi & 1);
+        cs.store16(&tmC, &tmC2, m0w, n0, p.N, [&](int j, int col, bool col_ok, uint32_t* v, uint32_t* vb) {
+          const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
-        for (int c = 0; c < BN / 64; ++c) {
-          if (n0 + 64 * c >= p.N) break;       // N % 32 == 0: the last chunk may be half inside N; TMA clips the rest
-          uint8_t* buf = epi + (2 * wg + (TWO ? 0 : (ep & 1))) * kEpiBufBytes;
-          const uint32_t row_addr = smem_u32(buf) + lrow * 128;
-#pragma unroll
-          for (int jp = 0; jp < 4; ++jp) {     // column groups j = 8c + 2jp + q, q = 0, 1: matrix 2q + h holds rows lr0 + 8h
-            uint32_t v[4], vb[4];
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-              const int j = 8 * c + 2 * jp + q, col = n0 + 8 * j + 2 * cq;
-              const bool col_ok = col < p.N;
-              const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-                if (p.bias) { f0 += b2.x; f1 += b2.y; }
-                if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
-                uint32_t val = pack2<BF16>(f0, f1);
-                if constexpr (EPI == B200_EPI_BIAS_ADD16 || EPI == B200_EPI_BIAS_MUL16) {
-                  const int row = m0w + lr0 + 8 * h;
-                  const uint32_t side = (row < p.M && col_ok)
-                      ? __ldg(reinterpret_cast<const uint32_t*>(p.add16) + (static_cast<size_t>(row) * p.N + col) / 2) : 0u;
-                  const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(side);
-                  // + shortcut, both already rounded to 16 bits like the reference
-                  if constexpr (EPI == B200_EPI_BIAS_ADD16) val = pack2<BF16>(a.x + r.x, a.y + r.y);
-                  // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
-                  if constexpr (EPI == B200_EPI_BIAS_MUL16) val = pack2<BF16>(a.x * r.x, a.y * r.y);
-                }
-                if constexpr (TWO) {           // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
-                  const float2 a = unpack2<BF16>(val);
-                  vb[2 * q + h] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
-                }
-                v[2 * q + h] = val;
-              }
+          for (int h = 0; h < 2; ++h) {
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            if (p.bias) { f0 += b2.x; f1 += b2.y; }
+            if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+            uint32_t val = pack2<BF16>(f0, f1);
+            if constexpr (EPI == B200_EPI_BIAS_ADD16 || EPI == B200_EPI_BIAS_MUL16) {
+              const int row = m0w + cs.lr0 + 8 * h;
+              const uint32_t side = (row < p.M && col_ok)
+                  ? __ldg(reinterpret_cast<const uint32_t*>(p.add16) + (static_cast<size_t>(row) * p.N + col) / 2) : 0u;
+              const float2 a = unpack2<BF16>(val), r = unpack2<BF16>(side);
+              // + shortcut, both already rounded to 16 bits like the reference
+              if constexpr (EPI == B200_EPI_BIAS_ADD16) val = pack2<BF16>(a.x + r.x, a.y + r.y);
+              // gated feed-forward: (h wi_1^T) * gelu(h wi_0^T), the second factor read back in 16 bits
+              if constexpr (EPI == B200_EPI_BIAS_MUL16) val = pack2<BF16>(a.x * r.x, a.y * r.y);
             }
-            // this lane's row holds column group 2jp + (mi >> 1) in 16-byte unit (2jp + (mi >> 1)) ^ (lrow % 8)
-            const uint32_t unit = ((2 * jp + (mi >> 1)) ^ (lane & 7)) << 4;
-            stmatrix_x4(row_addr + unit, v[0], v[1], v[2], v[3]);
-            if constexpr (TWO) stmatrix_x4(row_addr + kEpiBufBytes + unit, vb[0], vb[1], vb[2], vb[3]);
+            if constexpr (C::TWO_OUT) {      // training, fc1: keep the pre-activation u (out16) AND write gelu(u) (out16b)
+              const float2 a = unpack2<BF16>(val);
+              vb[h] = pack2<BF16>(gelu_tanh(a.x), gelu_tanh(a.y));
+            }
+            v[h] = val;
           }
-          fence_proxy_async_smem();            // the writes above -> visible to TMA
-          epi_bar(wg);
-          if (te == 0) {
-            tma_store_2d(&tmC, buf, n0 + 64 * c, m0w);
-            if constexpr (TWO) tma_store_2d(&tmC2, buf + kEpiBufBytes, n0 + 64 * c, m0w);
-            tma_store_commit();
-            // TWO rewrites both buffers every chunk; otherwise the previous chunk has been read out of the other buffer ...
-            if constexpr (TWO) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
-          }
-          epi_bar(wg);                         // ... which may now be rewritten
-          ++ep;
-        }
+        });
       }
     }
-    // every store / reduce-add of this warpgroup has been performed before the CTA retires, so the writes are complete with
-    // the grid, as a PDL-launched successor's griddepcontrol.wait expects
-    if (te == 0) tma_store_wait_all<0>();
+    cs.finish();
   }
 
   cluster_sync_all();   // the peer may still multicast into our smem / arrive on our barriers until it is done too
@@ -509,11 +582,19 @@ int pick_block_n(int M, int N, int K, bool resid, int sms) {
   return best;
 }
 
-// The scheduling decisions of one launch (shared by launch_gemm and the schedule dump the CPU tests read).
+// The scheduling decisions of one launch (shared by launch_gemm and the schedule dump the CPU tests read).  mn: the
+// operand layout of gemm_kernel (0 K-major, 2 dgrad, 3 wgrad).
 struct GemmPlan { int bn, pairs, pair_tiles, num_kb, streamk; };
-GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool split_small = false) {
+GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, int mn = 0) {
   GemmPlan g;
-  g.bn = block_n ? block_n : pick_block_n(M, N, K, resid, sms);
+  g.bn = block_n;
+  if (g.bn == 0) {
+    g.bn = pick_block_n(M, N, K, resid, sms);
+    if (mn != 0 && g.bn == 192) g.bn = (N % 256 == 0 || N > 1024) ? 256 : 128;   // W chunks are 64 wide per CTA: 128 or 256 only
+    // weight gradients: 256-wide tiles for every output of at least 256 columns (the tiles are split along K anyway, so
+    // the wider tile only halves the A traffic)
+    if (mn == 3 && N >= 256) g.bn = 256;
+  }
   const int num_m = (M + BM - 1) / BM, num_n = (N + g.bn - 1) / g.bn;
   g.pair_tiles = ((num_m + 1) / 2) * num_n;
   const int grid = 2 * g.pair_tiles < sms ? 2 * g.pair_tiles : (sms & ~1);   // whole clusters of 2
@@ -523,7 +604,7 @@ GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool s
   // weight gradients: a small output (fewer tiles than CTA pairs) under a very long contraction (K = tokens).  All tiles are
   // streamed: the (tile, k-block) units are cut into one equal share per pair, a tile's partial sums are reduce-added in k
   // order through the same flags (a chain of waits only ever points from pair p+1 to pair p, and every pair is resident).
-  if (split_small && resid && g.pair_tiles <= sms / 2 && g.pair_tiles % (sms / 2) != 0 &&
+  if (mn == 3 && resid && g.pair_tiles <= sms / 2 && g.pair_tiles % (sms / 2) != 0 &&
       static_cast<long long>(g.pair_tiles) * g.num_kb >= static_cast<long long>(sms / 2) * kStreamKMinKb) {
     g.pairs = sms / 2;
     g.streamk = 1;
@@ -531,18 +612,37 @@ GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, bool s
   return g;
 }
 
+// GemmDev with the problem and its grid of BM x bn tiles set, every other field zero
+GemmDev gemm_dev(int M, int N, int K, int bn) {
+  GemmDev p{};
+  p.M = M; p.N = N; p.K = K;
+  p.num_m = (M + BM - 1) / BM;
+  p.num_n = (N + bn - 1) / bn;
+  return p;
+}
+
+// a 16-bit [M, N] row-major output: one 64-row x 128-byte box (64 columns) per staging buffer; the callers' alignment
+// checks and N % 32 == 0 give TMA its 16-byte base and row stride
+int make_out16_map(CUtensorMap* m, void* out, int M, int N) {
+  const uint64_t dims[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(M)};
+  const uint64_t str[1] = {static_cast<uint64_t>(N) * 2};
+  const uint32_t box[2] = {64, 64};
+  return make_tmap_16bit(m, out, 2, dims, str, box, TMAP_SW_128);
+}
+
 // ---------------------------------------------------------------------------------------------------- FP8 (e4m3) GEMM
 // out16 = epi(s_a[row] * s_w[col] * (A8 . W8^T) + bias) for QKV and fc1 of the sampling forward: A8 and s_a come from
 // the e4m3 instance of ln_modulate (one scale per token), W8 and s_w from quantize_rows_e4m3 (one per output channel).
-// The mainloop is gemm_kernel's with K-major operands: CTA pairs, the multicast W half, 128B swizzle, the TMA producer
-// warpgroup.  A 128-byte swizzle row now holds 128 elements, so one stage is one 128-wide k-block with the same bytes as a
-// 16-bit stage, and a k-block is four m64nNk32 e4m3 wgmma whose descriptors advance 32 bytes each, as the 16-bit k16 steps
-// do.  K need not be a multiple of 128: the last k-block's columns past K are zero-filled by TMA (which still counts the
-// whole box toward the barrier's bytes).
+// It runs on the shared pieces above with K-major operands: prologue, pair tiles, TMA producer, stage bookkeeping and the
+// 16-bit epilogue.  Its own are the k-block and the output value.  A 128-byte swizzle row holds 128 e4m3 elements, so
+// one stage is one 128-wide k-block with the same bytes as a 16-bit stage, and a k-block is four m64nNk32 e4m3 wgmma whose
+// descriptors advance 32 bytes each, as the 16-bit k16 steps do.  K need not be a multiple of 128: the last k-block's
+// columns past K are zero-filled by TMA (which still counts the whole box toward the barrier's bytes).
 // Accumulation: FP8 wgmma keeps fewer accumulator bits than fp32 (DESIGN.md §6, FP8 sampling path), so each k-block is
 // summed in registers of its own -- alternately acc0 and acc1, the k-block's first wgmma overwriting -- and added into the
 // fp32 total `sum` once the NEXT k-block's wgmma are in flight: the k-loop still waits with wgmma_wait<1>.  The three
 // 64-float fragments fit the consumers' 232 registers at BN = 128 only, so that is the one tile width.
+// Output value: ((sum * s_a[row]) * s_w[col]) + bias, each step rounded, then GELU for fc1.
 constexpr int BN8 = 128;
 constexpr int BK8 = 128;
 
@@ -554,79 +654,25 @@ fp8_linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   using C = Cfg<BN8, EPI>;
   static_assert(C::A_BYTES == BM * BK8 && C::B_BYTES == BN8 * BK8, "a stage holds one e4m3 k-block");
   static_assert(EPI == B200_EPI_BIAS || EPI == B200_EPI_BIAS_GELU, "16-bit output epilogues only");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + C::STAGES;
-
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 4);
-    }
-    fence_mbar_init();
-  }
-  cluster_sync_all();
-  pdl_launch_dependents();
-
-  const uint32_t rank = cluster_ctarank();
-  const int num_pair_m = (p.num_m + 1) / 2;
-  const int num_tiles = num_pair_m * p.num_n;
-  const int my_pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
+  const Pipeline<C> pl = gemm_prologue<C>(&tmA, &tmB, &tmC);
+  const PairTiles<BN8> pt(p);
   const int num_kb = (p.K + BK8 - 1) / BK8;
 
   if (warp < 4) {
-    // ------------------------------------------------------------------ TMA producer (as gemm_kernel's)
-    setmaxnreg_dec<kProducerRegs>();
-    if (threadIdx.x == 0) {
-      pdl_wait();
-      TileSched sched(my_pair, num_pairs, num_tiles, num_kb, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int tile, kb0, kb1;
-      while (sched.next(tile, kb0, kb1)) {
-        const int m_blk = 2 * (tile / p.num_n) + static_cast<int>(rank), n_blk = tile % p.num_n;
-        const int w_row0 = n_blk * BN8 + static_cast<int>(rank) * (BN8 / 2);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
-          uint8_t* sa = smem + stage * C::STAGE_BYTES;
-          tma_load_2d(sa, &tmA, &full[stage], kb * BK8, m_blk * BM);
-          tma_load_2d_mcast(sa + C::A_BYTES + rank * (C::B_BYTES / 2), &tmB, &full[stage], kb * BK8, w_row0, 0x3);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
+    produce(pl, pt, num_kb, false, [&](uint8_t* sa, uint64_t* bar, int m_blk, int w_row0, int kb) {
+      tma_load_2d(sa, &tmA, bar, kb * BK8, m_blk * BM);
+      tma_load_2d_mcast(sa + C::A_BYTES + pt.rank * (C::B_BYTES / 2), &tmB, bar, kb * BK8, w_row0, 0x3);
+    });
   } else {
-    // ------------------------------------------------------------------ MMA + epilogue: warpgroups 1, 2 (64 rows each)
-    setmaxnreg_inc<kConsumerRegs>();
-    pdl_wait();
-    const int wg = (warp >> 2) - 1;
-    const int te = threadIdx.x & 127;
-    const int w4 = te >> 5, g = lane >> 2, cq = lane & 3;
-    const uint32_t empty_peer = mapa_u32(&empty[0], rank ^ 1u);
-    int stage = 0;
-    uint32_t phase = 0;
+    Consumer<C> cs(pl, pt.rank, (warp >> 2) - 1);
     float acc0[BN8 / 2], acc1[BN8 / 2], sum[BN8 / 2];
-    uint8_t* epi = smem + C::EPI_OFF;
-    int ep = 0;
-    int prev = -1;                            // slot of the k-block whose wgmma may still be running
-    // one k-block into `cur`; once the previous k-block's wgmma have completed, its slot is released in both CTAs and its
-    // partial sum `done` is added into `sum`
+    // one k-block into `cur`; once the previous k-block's wgmma have completed, its slot is released and its partial sum
+    // `done` is added into `sum`
     auto kblock = [&](float (&cur)[BN8 / 2], float (&done)[BN8 / 2]) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES), sb = sa + C::A_BYTES;
+      const uint32_t sa = cs.wait(), sb = sa + C::A_BYTES;
       wgmma_fence();
-      const uint64_t da = gmma_desc(sa + wg * 8192, 16, 1024, GMMA_LAYOUT_SW128);
+      const uint64_t da = gmma_desc(sa + cs.wg * 8192, 16, 1024, GMMA_LAYOUT_SW128);
       const uint64_t db = gmma_desc(sb, 16, 1024, GMMA_LAYOUT_SW128);
 #pragma unroll
       for (int k = 0; k < BK8 / 32; ++k)
@@ -634,30 +680,21 @@ fp8_linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_commit();
       wgmma_wait<1>();
       reg_fence(done);
-      if (prev >= 0 && te == 0) {
-        mbar_arrive(&empty[prev]);
-        mbar_arrive_cluster(empty_peer + prev * 8);
-      }
-      prev = stage;
-      if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      cs.release_prev();
 #pragma unroll
       for (int i = 0; i < BN8 / 2; ++i) sum[i] += done[i];
     };
     auto drain = [&](float (&cur)[BN8 / 2]) {
       wgmma_wait<0>();
       reg_fence(cur);
-      if (te == 0) {
-        mbar_arrive(&empty[prev]);
-        mbar_arrive_cluster(empty_peer + prev * 8);
-      }
+      cs.release_last();
 #pragma unroll
       for (int i = 0; i < BN8 / 2; ++i) sum[i] += cur[i];
     };
-    TileSched sched(my_pair, num_pairs, num_tiles, num_kb, false);
+    TileSched sched = pt.sched(num_kb, false);
     int tile, kb0, kb1;
     while (sched.next(tile, kb0, kb1)) {
-      const int m0 = (2 * (tile / p.num_n) + static_cast<int>(rank)) * BM, n0 = (tile % p.num_n) * BN8;
-      prev = -1;                              // the previous tile's last slot was released by its drain
+      const int m0 = pt.m_blk(tile) * BM, n0 = pt.n0(tile);
 #pragma unroll
       for (int i = 0; i < BN8 / 2; ++i) { sum[i] = 0.f; acc1[i] = 0.f; }
       for (int kb = kb0;;) {                  // k-blocks alternate between acc0 and acc1 (acc1 = 0 before the first)
@@ -667,54 +704,26 @@ fp8_linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (++kb == kb1) { drain(acc1); break; }
       }
 
-      // the 16-bit epilogue of gemm_kernel: v = (sum * s_a[row]) * s_w[col] + bias (each step rounded), then GELU for fc1
-      const int m0w = m0 + wg * 64;
-      const int lr0 = w4 * 16 + g;
+      const int m0w = m0 + cs.wg * 64;
       float sa_row[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = m0w + lr0 + 8 * h;
+        const int row = m0w + cs.lr0 + 8 * h;
         sa_row[h] = row < p.M ? __ldg(a_scale + row) : 0.f;   // rows past M are clipped by the TMA store
       }
-      const int mi = lane >> 3;
-      const int lrow = w4 * 16 + (lane & 7) + 8 * (mi & 1);
+      cs.store16(&tmC, nullptr, m0w, n0, p.N, [&](int j, int col, bool col_ok, uint32_t* v, uint32_t*) {
+        const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+        const float2 s2 = col_ok ? __ldg(reinterpret_cast<const float2*>(w_scale + col)) : make_float2(0.f, 0.f);
 #pragma unroll
-      for (int c = 0; c < BN8 / 64; ++c) {
-        if (n0 + 64 * c >= p.N) break;
-        uint8_t* buf = epi + (2 * wg + (ep & 1)) * kEpiBufBytes;
-        const uint32_t row_addr = smem_u32(buf) + lrow * 128;
-#pragma unroll
-        for (int jp = 0; jp < 4; ++jp) {
-          uint32_t v[4];
-#pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const int j = 8 * c + 2 * jp + q, col = n0 + 8 * j + 2 * cq;
-            const bool col_ok = col < p.N;
-            const float2 b2 = (p.bias && col_ok) ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
-            const float2 s2 = col_ok ? __ldg(reinterpret_cast<const float2*>(w_scale + col)) : make_float2(0.f, 0.f);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              float f0 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h], sa_row[h]), s2.x), b2.x);
-              float f1 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h + 1], sa_row[h]), s2.y), b2.y);
-              if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
-              v[2 * q + h] = pack2<BF16>(f0, f1);
-            }
-          }
-          const uint32_t unit = ((2 * jp + (mi >> 1)) ^ (lane & 7)) << 4;
-          stmatrix_x4(row_addr + unit, v[0], v[1], v[2], v[3]);
+        for (int h = 0; h < 2; ++h) {
+          float f0 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h], sa_row[h]), s2.x), b2.x);
+          float f1 = __fadd_rn(__fmul_rn(__fmul_rn(sum[4 * j + 2 * h + 1], sa_row[h]), s2.y), b2.y);
+          if constexpr (EPI == B200_EPI_BIAS_GELU) { f0 = gelu_tanh(f0); f1 = gelu_tanh(f1); }
+          v[h] = pack2<BF16>(f0, f1);
         }
-        fence_proxy_async_smem();
-        epi_bar(wg);
-        if (te == 0) {
-          tma_store_2d(&tmC, buf, n0 + 64 * c, m0w);
-          tma_store_commit();
-          tma_store_wait_read<1>();
-        }
-        epi_bar(wg);
-        ++ep;
-      }
+      });
     }
-    if (te == 0) tma_store_wait_all<0>();
+    cs.finish();
   }
 
   cluster_sync_all();
@@ -735,12 +744,8 @@ int gemm_schedule(int M, int N, int K, int epilogue, int block_n, int sms, int* 
                   int* segments, int max_segments, int wgrad) {
   B200_REQUIRE(M > 0 && N > 0 && K > 0 && K % BK == 0 && sms >= 2, B200_ERR_SHAPE, "gemm_schedule: bad arguments");
   B200_REQUIRE(block_n == 0 || block_n == 128 || block_n == 192 || block_n == 256, B200_ERR_UNSUPPORTED, "gemm_schedule: block_n %d", block_n);
-  if (wgrad && block_n == 0) {               // the tile-width rule launch_gemm applies to weight gradients (mn_major == 3)
-    block_n = pick_block_n(M, N, K, true, sms);
-    if (block_n == 192) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
-    if (N >= 256) block_n = 256;
-  }
-  const GemmPlan g = plan_gemm(M, N, K, epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, wgrad != 0);
+  // wgrad: the schedule launch_gemm gives a weight gradient (both operands transposed)
+  const GemmPlan g = plan_gemm(M, N, K, epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, wgrad ? 3 : 0);
   if (bn_out) *bn_out = g.bn;
   if (pairs_out) *pairs_out = g.pairs;
   if (streamk_out) *streamk_out = g.streamk;
@@ -789,21 +794,13 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
 
   B200_REQUIRE(a.block_n == 0 || a.block_n == 128 || a.block_n == 192 || a.block_n == 256, B200_ERR_UNSUPPORTED,
                "gemm: block_n must be 128, 192 or 256 (got %d)", a.block_n);
-  int block_n = a.block_n;
   if (a.mn_major) {
     B200_REQUIRE((a.mn_major == 2 || a.mn_major == 3) && a.conv_taps == 0 && (!(a.mn_major & 1) || a.M % 8 == 0) &&
                      (!(a.mn_major & 2) || a.N % 128 == 0) && (a.block_n == 0 || a.block_n == 128 || a.block_n == 256),
                  B200_ERR_UNSUPPORTED, "gemm (transposed operands): mn_major 2 or 3, M %% 8 == 0, N %% 128 == 0, block_n 128 or 256 (M=%d N=%d)",
                  a.M, a.N);
-    if (block_n == 0) {
-      block_n = pick_block_n(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, sms);
-      if (block_n == 192) block_n = (a.N % 256 == 0 || a.N > 1024) ? 256 : 128;     // W chunks are 64 wide per CTA: 128 or 256 only
-      // weight gradients: 256-wide tiles for every output of at least 256 columns (the tiles are split along K anyway, so
-      // the wider tile only halves the A traffic)
-      if (a.mn_major == 3) block_n = a.N >= 256 ? 256 : block_n;
-    }
   }
-  const GemmPlan plan = plan_gemm(a.M, a.N, a.K, a.epilogue == B200_EPI_GATE_RESIDUAL, block_n, sms, a.mn_major == 3);
+  const GemmPlan plan = plan_gemm(a.M, a.N, a.K, resid, a.block_n, sms, a.mn_major);
   const int bn = plan.bn;
 
   GemmMaps tm;
@@ -847,26 +844,20 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
       const uint32_t boxB[2] = {BK, static_cast<uint32_t>(bn / 2)};   // each CTA of the pair fetches half and multicasts it
       B200_TRY(make_tmap_16bit(&tmB, a.W, 2, dimsB, strB, boxB, TMAP_SW_128));
     }
-    // the output, [M, N] row-major: one 64-row x 128-byte box per staging buffer (32 fp32 or 64 16-bit columns); the
-    // alignment checks above and N % 32 == 0 give TMA its 16-byte base and row stride
-    const uint64_t dimsC[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
+    // the output, [M, N] row-major: one 64-row x 128-byte box per staging buffer (32 fp32 or 64 16-bit columns)
     if (resid) {
+      const uint64_t dimsC[2] = {static_cast<uint64_t>(a.N), static_cast<uint64_t>(a.M)};
       const uint64_t strC[1] = {static_cast<uint64_t>(a.N) * 4};
       const uint32_t boxC[2] = {32, 64};
       B200_TRY(make_tmap(&tm.c, a.resid, 4, 2, dimsC, strC, boxC, TMAP_SW_128));
       tm.c2 = tm.c;
     } else {
-      const uint64_t strC[1] = {static_cast<uint64_t>(a.N) * 2};
-      const uint32_t boxC[2] = {64, 64};
-      B200_TRY(make_tmap_16bit(&tm.c, a.out16, 2, dimsC, strC, boxC, TMAP_SW_128));
-      if (a.epilogue == B200_EPI_BIAS_GELU_BOTH) B200_TRY(make_tmap_16bit(&tm.c2, a.out16b, 2, dimsC, strC, boxC, TMAP_SW_128));
+      B200_TRY(make_out16_map(&tm.c, a.out16, a.M, a.N));
+      if (a.epilogue == B200_EPI_BIAS_GELU_BOTH) B200_TRY(make_out16_map(&tm.c2, a.out16b, a.M, a.N));
       else tm.c2 = tm.c;
     }
   }
-  GemmDev p;
-  p.M = a.M; p.N = a.N; p.K = a.K;
-  p.num_m = (a.M + BM - 1) / BM;
-  p.num_n = (a.N + bn - 1) / bn;
+  GemmDev p = gemm_dev(a.M, a.N, a.K, bn);
   p.bias = a.bias;
   p.out16 = a.out16;
   p.gate = a.gate;
@@ -926,15 +917,9 @@ int launch_linear_e4m3(const void* A8, const float* a_scale, const void* W8, con
     const uint64_t dimsB[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
     const uint32_t boxB[2] = {BK8, BN8 / 2};
     B200_TRY(make_tmap(&tm.b, W8, 1, 2, dimsB, strA, boxB, TMAP_SW_128));
-    const uint64_t dimsC[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(M)};
-    const uint64_t strC[1] = {static_cast<uint64_t>(N) * 2};
-    const uint32_t boxC[2] = {64, 64};
-    B200_TRY(make_tmap_16bit(&tm.c, out16, 2, dimsC, strC, boxC, TMAP_SW_128));
+    B200_TRY(make_out16_map(&tm.c, out16, M, N));
   }
-  GemmDev p{};
-  p.M = M; p.N = N; p.K = K;
-  p.num_m = (M + BM - 1) / BM;
-  p.num_n = (N + BN8 - 1) / BN8;
+  GemmDev p = gemm_dev(M, N, K, BN8);
   p.bias = bias;
   p.out16 = out16;
   p.rows_per_batch = 1;
