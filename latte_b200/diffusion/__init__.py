@@ -346,19 +346,18 @@ class _FusedLoss(torch.autograd.Function):
                                                 torch.cuda.current_stream(dev).cuda_stream)
         _lib.check(rc, "b200_training_loss")
         n = float(F * Cc * hw)
-        ctx.dmo, ctx.Cc = dmo, Cc
+        # saved, not kept on ctx: autograd frees it after the first backward, so a second backward through a freed graph
+        # raises autograd's own error, and one through a retained graph adds the gradient again, as torch's loss would
+        if need_grad:
+            ctx.save_for_backward(dmo)
         return sums[0] / n, sums[1] / (n * float(np.log(2.0)))
 
     @staticmethod
     def backward(ctx, g_mse, g_vb):
-        dmo, Cc = ctx.dmo, ctx.Cc
-        if dmo is None:
-            return (None,) * 6
-        ctx.dmo = None
-        shape = (-1, 1, 1, 1, 1)
-        dmo[:, :, :Cc].mul_(g_mse.reshape(shape))
-        dmo[:, :, Cc:].mul_(g_vb.reshape(shape))
-        return None, dmo, None, None, None, None
+        (dmo,) = ctx.saved_tensors
+        B, F = dmo.shape[:2]
+        scale = torch.stack((g_mse, g_vb), dim=1).reshape(B, 1, 2, 1, 1)
+        return None, (dmo.reshape(B, F, 2, -1, dmo.shape[-1]) * scale).reshape(dmo.shape), None, None, None, None
 
 
 def create_diffusion(timestep_respacing, noise_schedule="linear", use_kl=False, sigma_small=False, predict_xstart=False,

@@ -41,7 +41,7 @@ def t2v_train_forward(sd, cfg: T2VConfig, x, t, text, use_image_num, text_mask=N
     xf = x.permute(0, 2, 1, 3, 4).reshape(B * Fa, C, Hh, Ww).to(dtype)                     # :731
     patches = xf.reshape(B * Fa, C, Hh // p, p, Ww // p, p).permute(0, 2, 4, 1, 3, 5).reshape(B * Fa, N, C * p * p)
     h = patches @ sd["pos_embed.proj.weight"].to(dtype).reshape(D, -1).t() + sd["pos_embed.proj.bias"].to(dtype)
-    h = h + pos_embed_table(cfg).to(dtype)
+    h = h + pos_embed_table(cfg).to(device=h.device, dtype=dtype)
     ts, emb = adaln_single(sd, t, dtype)                                                    # :782-784
 
     def per_frame(a):

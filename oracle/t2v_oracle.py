@@ -190,7 +190,7 @@ def t2v_forward(sd, cfg: T2VConfig, x, t, text, dtype=torch.float32, enable_temp
     xf = x.permute(0, 2, 1, 3, 4).reshape(B * Fr, C, Hh, Ww).to(dtype)
     patches = xf.reshape(B * Fr, C, Hh // p, p, Ww // p, p).permute(0, 2, 4, 1, 3, 5).reshape(B * Fr, N, C * p * p)
     h = patches @ sd["pos_embed.proj.weight"].to(dtype).reshape(D, -1).t() + sd["pos_embed.proj.bias"].to(dtype)
-    h = h + pos_embed_table(cfg).to(dtype)
+    h = h + pos_embed_table(cfg).to(device=h.device, dtype=dtype)
     # :782-784 adaln_single: emb = TimestepEmbedding(Timesteps(t)); ts = Linear(SiLU(emb))
     ts, emb = adaln_single(sd, t, dtype)
     # :789 caption projection, :798 repeat per frame
@@ -206,7 +206,7 @@ def t2v_forward(sd, cfg: T2VConfig, x, t, text, dtype=torch.float32, enable_temp
         if enable_temporal:
             h = h.reshape(B, Fr, N, D).permute(0, 2, 1, 3).reshape(B * N, Fr, D)            # :874
             if i == 0 and Fr > 1:
-                h = h + temp_pos_embed_table(cfg).to(dtype)                                  # :894-895
+                h = h + temp_pos_embed_table(cfg).to(device=h.device, dtype=dtype)          # :894-895
             h = temporal_block(sd, i, h, ts_tm, heads)                                      # :897-905
             h = h.reshape(B, N, Fr, D).permute(0, 2, 1, 3).reshape(B * Fr, N, D)            # :907
     # :918-924 output head
