@@ -7,7 +7,7 @@ copy must not alias another instance's buffers, so `copy.deepcopy(model)` (the E
 """
 from __future__ import annotations
 
-import torch
+from . import ops
 
 
 class DeviceCacheMixin:
@@ -26,6 +26,6 @@ class DeviceCacheMixin:
         """Device address of `need` bytes of scratch on a 1024-byte boundary, inside `_workspace` (reallocated when it is too
         small or on another device)."""
         ws = self._workspace
-        if ws is None or ws.numel() < need + 1024 or ws.device != device:
-            ws = self._workspace = torch.empty(need + 1024, dtype=torch.uint8, device=device)
-        return (ws.data_ptr() + 1023) // 1024 * 1024
+        if ws is None or ws[0].numel() < need + 1024 or ws[0].device != device:
+            ws = self._workspace = ops.scratch(need, device)
+        return ws[1]

@@ -24,10 +24,9 @@ import os
 import numpy as np
 import torch
 
-from latte_b200 import _lib   # absolute: this package is also importable as top-level `diffusion` through a symlink (INTEGRATION.md)
+from latte_b200 import _lib, ops   # absolute: this package is also importable as top-level `diffusion` through a symlink (INTEGRATION.md)
 
 DDPM, DDIM = 0, 1
-_DT = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 
 def _space_timesteps(num_timesteps: int, section_counts) -> set:
@@ -128,8 +127,6 @@ class SpacedDiffusion:
         hw = int(np.prod(x.shape[3:]))
         if tuple(model_output.shape) != (B, F, 2 * C_, *x.shape[3:]):
             raise ValueError(f"model output {tuple(model_output.shape)} != {(B, F, 2 * C_, *x.shape[3:])} (learn_sigma layout)")
-        if model_output.dtype not in _DT:
-            raise TypeError(f"model output dtype {model_output.dtype} unsupported")
         x = x.float().contiguous()
         model_output = model_output.contiguous()
         t = t.to(device=x.device, dtype=torch.int64).contiguous()
@@ -138,12 +135,9 @@ class SpacedDiffusion:
         tab = self._state(x.device, B, eta)[0]
         outs = {k: torch.empty_like(x) for k in want}
         ptr = lambda k: outs[k].data_ptr() if k in outs else None   # noqa: E731
-        lib = _lib.load()
-        rc = lib.b200_sampler_step(C.byref(tab), method, int(bool(clip_denoised)), t.data_ptr(), x.data_ptr(),
-                                   model_output.data_ptr(), _DT[model_output.dtype], noise.data_ptr() if noise is not None else None,
-                                   B, F, C_, hw, ptr("sample"), ptr("pred_xstart"), ptr("mean"), ptr("log_variance"),
-                                   torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(rc, "b200_sampler_step")
+        ops.call("b200_sampler_step", x.device, C.byref(tab), method, int(bool(clip_denoised)), t.data_ptr(), x.data_ptr(),
+                 model_output.data_ptr(), ops._kind(model_output), noise.data_ptr() if noise is not None else None,
+                 B, F, C_, hw, ptr("sample"), ptr("pred_xstart"), ptr("mean"), ptr("log_variance"))
         return outs
 
     def _call_model(self, model, x, t, model_kwargs, mapped=None, traj=None):
@@ -340,11 +334,8 @@ class _FusedLoss(torch.autograd.Function):
         sums = torch.empty(2, B, dtype=torch.float32, device=dev)
         need_grad = ctx.needs_input_grad[1]
         dmo = torch.empty_like(mo) if need_grad else None
-        with torch.cuda.device(dev):
-            rc = _lib.load().b200_training_loss(C.byref(tab), tt.data_ptr(), x0.data_ptr(), x_t.data_ptr(), noise.data_ptr(), mo.data_ptr(),
-                                                B, F, Cc, hw, sums.data_ptr(), dmo.data_ptr() if need_grad else None,
-                                                torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(rc, "b200_training_loss")
+        ops.call("b200_training_loss", dev, C.byref(tab), tt.data_ptr(), x0.data_ptr(), x_t.data_ptr(), noise.data_ptr(),
+                 mo.data_ptr(), B, F, Cc, hw, sums.data_ptr(), dmo.data_ptr() if need_grad else None)
         n = float(F * Cc * hw)
         # saved, not kept on ctx: autograd frees it after the first backward, so a second backward through a freed graph
         # raises autograd's own error, and one through a retained graph adds the gradient again, as torch's loss would

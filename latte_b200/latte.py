@@ -22,7 +22,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, ops
 from .ops import quantize_rows_e4m3
 from ._cache import DeviceCacheMixin
 from .training import GradientCheckpointingMixin
@@ -320,7 +320,6 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
                 raise NotImplementedError("latte_b200: forward_with_cfg / trajectory conditioning are sampling-only; train through forward()")
             return self._run_train(x, t, y)
         self._check_input(x)
-        lib = _lib.load()
         dev = x.device
         B = x.shape[0]
         with torch.cuda.device(dev):
@@ -336,17 +335,14 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
                 mod = traj[int(trajectory_step)]                    # [B, depth*6D + 2D] rows precomputed for this step
                 if mod.shape[0] != B or mod.device != dev:
                     raise ValueError("precomputed conditioning does not match this batch")
-            need = lib.b200_latte_workspace_bytes(C.byref(shape), B)
-            if need == 0:
-                raise RuntimeError("latte_b200: unsupported configuration: " + _lib.last_error())
+            need = ops.workspace_bytes("b200_latte_workspace_bytes", C.byref(shape), B)
             if (self.use_cuda_graphs and not torch.is_grad_enabled() and not torch.cuda.is_current_stream_capturing()
                     and not _lib.profiling_enabled()):
-                out = self._run_graphed(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev)
+                out = self._run_graphed(shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev)
             else:
                 out = torch.empty(B, self.num_frames, self.out_channels, self.input_size, self.input_size,
                                   dtype=torch.float32, device=dev)
-                self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need,
-                             torch.cuda.current_stream(dev).cuda_stream)
+                self._launch(shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need, dev)
         pd = self.blocks[0].attn.qkv.weight.dtype
         return out if pd == torch.float32 else out.to(pd)
 
@@ -362,27 +358,24 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         self._check_input(x)
         dev = x.device
         _lib.load()
-        od, ops = training.native_backend(self, self.blocks[0].attn.qkv.weight.dtype)
+        od, backend = training.native_backend(self, self.blocks[0].attn.qkv.weight.dtype)
         B = x.shape[0]
         tt = t.to(device=dev, dtype=torch.int64)
         yy = self._labels(y, B, dev)
         with torch.autocast("cuda", enabled=False):
             c = training.conditioning(self, tt, yy)
-            return training.train_forward(self, ops, od, x.float(), c)
+            return training.train_forward(self, backend, od, x.float(), c)
 
-    def _launch(self, lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, base, need, stream):
-        """ONE C-ABI call = the whole forward (206 kernel launches for XL/2 with CFG) enqueued on `stream`."""
+    def _launch(self, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, base, need, dev):
+        """ONE C-ABI call = the whole forward (206 kernel launches for XL/2 with CFG) enqueued on `dev`'s current stream."""
         if mod is not None:
-            rc = lib.b200_latte_forward_conditioned(C.byref(shape), C.byref(w), xf.data_ptr(), mod.data_ptr(), B, int(use_cfg),
-                                                    float(cfg_scale), out.data_ptr(), base, need, stream)
-            _lib.check(rc, "b200_latte_forward_conditioned")
+            ops.call("b200_latte_forward_conditioned", dev, C.byref(shape), C.byref(w), xf.data_ptr(), mod.data_ptr(), B,
+                     int(use_cfg), float(cfg_scale), out.data_ptr(), base, need)
         else:
-            rc = lib.b200_latte_forward(C.byref(shape), C.byref(w), xf.data_ptr(), tt.data_ptr(),
-                                        yy.data_ptr() if yy is not None else None, B, int(use_cfg), float(cfg_scale),
-                                        out.data_ptr(), base, need, stream)
-            _lib.check(rc, "b200_latte_forward")
+            ops.call("b200_latte_forward", dev, C.byref(shape), C.byref(w), xf.data_ptr(), tt.data_ptr(),
+                     yy.data_ptr() if yy is not None else None, B, int(use_cfg), float(cfg_scale), out.data_ptr(), base, need)
 
-    def _run_graphed(self, lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev):
+    def _run_graphed(self, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, need, dev):
         """CUDA-graph replay of the forward.  The C-ABI call neither allocates nor synchronises and keeps no host-side launch
         state, so its launch sequence can be captured once per call signature and replayed with the inputs copied into
         fixed buffers: the per-step host cost drops from ~200 launches to three small copies and one graph launch.
@@ -395,21 +388,18 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
             self._graphs[key] = {"graph": None}
             out = torch.empty(B, self.num_frames, self.out_channels, self.input_size, self.input_size,
                               dtype=torch.float32, device=dev)
-            self._launch(lib, shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need,
-                         torch.cuda.current_stream(dev).cuda_stream)
+            self._launch(shape, w, xf, tt, yy, mod, B, use_cfg, cfg_scale, out, self._aligned_workspace(need, dev), need, dev)
             return out
         if st["graph"] is None:
-            st["ws"] = torch.empty(need + 1024, dtype=torch.uint8, device=dev)     # this graph's own scratch
+            st["ws"], base = ops.scratch(need, dev)                                 # this graph's own scratch
             st["x"], st["t"] = torch.empty_like(xf), torch.empty_like(tt)
             st["y"] = torch.empty_like(yy) if yy is not None else None
             st["mod"] = torch.empty_like(mod) if mod is not None else None
             st["out"] = torch.empty(B, self.num_frames, self.out_channels, self.input_size, self.input_size,
                                     dtype=torch.float32, device=dev)
-            base = (st["ws"].data_ptr() + 1023) // 1024 * 1024
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._launch(lib, shape, w, st["x"], st["t"], st["y"], st["mod"], B, use_cfg, cfg_scale, st["out"], base, need,
-                             torch.cuda.current_stream(dev).cuda_stream)
+                self._launch(shape, w, st["x"], st["t"], st["y"], st["mod"], B, use_cfg, cfg_scale, st["out"], base, need, dev)
             st["graph"] = g
         st["x"].copy_(xf)
         st["t"].copy_(tt)
@@ -442,7 +432,6 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
         Evaluates all steps * B rows once (same kernels and arithmetic as inside forward -> bit-identical outputs) and keeps
         them on the device; `forward*(…, trajectory_step=i)` then skips the 446 MB/step adaLN weight stream.  Used by
         latte_b200.diffusion's loops; `clear_conditioning()` drops the cache."""
-        lib = _lib.load()
         dev = self.pos_embed.device
         if dev.type != "cuda":
             raise RuntimeError("latte_b200.Latte runs on CUDA (sm_90a) only; there is no CPU fallback")
@@ -456,18 +445,14 @@ class Latte(GradientCheckpointingMixin, DeviceCacheMixin, nn.Module):
                     raise ValueError("class-conditional model (extras=2) needs labels y")
                 yy = y.detach().to(device=dev, dtype=torch.int64).view(1, B).expand(steps, B).contiguous().view(-1)
             n = steps * B
-            row = lib.b200_latte_conditioning_bytes(C.byref(shape), 1) // 4
-            if row == 0:
-                raise RuntimeError("latte_b200: unsupported configuration: " + _lib.last_error())
+            row = ops.workspace_bytes("b200_latte_conditioning_bytes", C.byref(shape), 1) // 4
             mod = torch.empty(n * row + 256, dtype=torch.float32, device=dev)
             off = (-(mod.data_ptr() // 4)) % 256                      # 1024-byte aligned start
             mod = mod[off:off + n * row]
-            need = lib.b200_latte_conditioning_workspace_bytes(C.byref(shape), n)
-            ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
-            base = (ws.data_ptr() + 1023) // 1024 * 1024
-            rc = lib.b200_latte_conditioning(C.byref(shape), C.byref(w), tt.data_ptr(), yy.data_ptr() if yy is not None else None,
-                                             n, mod.data_ptr(), base, need, torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(rc, "b200_latte_conditioning")
+            need = ops.workspace_bytes("b200_latte_conditioning_workspace_bytes", C.byref(shape), n)
+            ws, base = ops.scratch(need, dev)
+            ops.call("b200_latte_conditioning", dev, C.byref(shape), C.byref(w), tt.data_ptr(),
+                     yy.data_ptr() if yy is not None else None, n, mod.data_ptr(), base, need)
             ws.record_stream(torch.cuda.current_stream(dev))
         self._trajectory = mod.view(steps, B, row)
         self._frozen = self._packed      # the loop's steps reuse this packing without re-walking the 293 parameters

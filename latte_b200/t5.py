@@ -18,7 +18,7 @@ from types import SimpleNamespace
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, ops
 from ._cache import DeviceCacheMixin
 
 MAX_LEN = 128
@@ -185,7 +185,6 @@ class T5EncoderModel(DeviceCacheMixin, nn.Module):
         if L > MAX_LEN:
             raise NotImplementedError(f"sequences longer than {MAX_LEN} tokens are not built (the pipeline uses 120)")
         dev = input_ids.device
-        lib = _lib.load()
         with torch.cuda.device(dev):
             shape, w, _, pos = self._pack()
             ids = torch.zeros(B, MAX_LEN, dtype=torch.int64, device=dev)
@@ -194,12 +193,9 @@ class T5EncoderModel(DeviceCacheMixin, nn.Module):
             keep = torch.ones(B, L, device=dev) if attention_mask is None else attention_mask.to(device=dev, dtype=torch.float32)
             bias[:, :L] = (1.0 - keep) * -1e30                                         # the extended attention mask
             out = torch.empty(B, MAX_LEN, self.config.d_model, dtype=torch.float32, device=dev)
-            need = lib.b200_t5_workspace_bytes(C.byref(shape), B)
-            if need == 0:
-                raise RuntimeError("latte_b200: unsupported T5 configuration: " + _lib.last_error())
-            rc = lib.b200_t5_encode(C.byref(shape), C.byref(w), ids.data_ptr(), bias.data_ptr(), pos.data_ptr(), B, out.data_ptr(),
-                                    self._aligned_workspace(need, dev), need, torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(rc, "b200_t5_encode")
+            need = ops.workspace_bytes("b200_t5_workspace_bytes", C.byref(shape), B)
+            ops.call("b200_t5_encode", dev, C.byref(shape), C.byref(w), ids.data_ptr(), bias.data_ptr(), pos.data_ptr(), B,
+                     out.data_ptr(), self._aligned_workspace(need, dev), need)
         pd = self.dtype
         res = out[:, :L].contiguous()
         res = res if pd == torch.float32 else res.to(pd)

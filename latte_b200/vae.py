@@ -14,7 +14,7 @@ from types import SimpleNamespace
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, ops
 from ._cache import DeviceCacheMixin
 
 
@@ -359,7 +359,6 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             raise NotImplementedError("AutoencoderKLTemporalDecoder.encode is outside the built path (the pipelines only decode with it)")
         if not x.is_cuda:
             raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_90a) only; there is no CPU fallback")
-        lib = _lib.load()
         dev = x.device
         n, ci, h, w = x.shape
         f = 2 ** (len(self.config.block_out_channels) - 1)
@@ -367,13 +366,9 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             e, _, _ = self._pack_encoder()
             xf = x.detach().to(torch.float32).contiguous()
             moments = torch.empty(n, 2 * self.config.latent_channels, h // f, w // f, dtype=torch.float32, device=dev)
-            need = lib.b200_vae_encode_workspace_bytes(C.byref(e), n, h, w)
-            if need == 0:
-                raise RuntimeError("latte_b200: unsupported VAE encode configuration: " + _lib.last_error())
-            base = self._aligned_workspace(need, dev)
-            rc = lib.b200_vae_encode(C.byref(e), xf.data_ptr(), n, h, w, moments.data_ptr(), base, need,
-                                     torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(rc, "b200_vae_encode")
+            need = ops.workspace_bytes("b200_vae_encode_workspace_bytes", C.byref(e), n, h, w)
+            ops.call("b200_vae_encode", dev, C.byref(e), xf.data_ptr(), n, h, w, moments.data_ptr(),
+                     self._aligned_workspace(need, dev), need)
         pd = self.dtype
         dist = DiagonalGaussianDistribution(moments if pd == torch.float32 else moments.to(pd))
         return AutoencoderKLOutput(latent_dist=dist) if return_dict else (dist,)
@@ -468,7 +463,6 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
         and required by AutoencoderKLTemporalDecoder (one clip per call: n == num_frames, as pipeline_latte.py:785-792 does)."""
         if not z.is_cuda:
             raise RuntimeError("latte_b200.AutoencoderKL runs on CUDA (sm_90a) only; there is no CPU fallback")
-        lib = _lib.load()
         dev = z.device
         n, cz, h, w = z.shape
         scale = 2 ** (len(self.config.block_out_channels) - 1)
@@ -476,19 +470,15 @@ class AutoencoderKL(DeviceCacheMixin, nn.Module):
             d, _ = self._pack()
             zf = z.detach().to(torch.float32).contiguous()
             out = torch.empty(n, self.config.out_channels, h * scale, w * scale, dtype=torch.float32, device=dev)
-            need = lib.b200_vae_workspace_bytes(C.byref(d), n, h, w)
-            if need == 0:
-                raise RuntimeError("latte_b200: unsupported VAE configuration: " + _lib.last_error())
+            need = ops.workspace_bytes("b200_vae_workspace_bytes", C.byref(d), n, h, w)
             base = self._aligned_workspace(need, dev)
             if self._temporal:
                 if num_frames is None:
                     raise ValueError("AutoencoderKLTemporalDecoder.decode needs num_frames")
-                rc = lib.b200_vae_decode_temporal(C.byref(d), zf.data_ptr(), n, h, w, int(num_frames), out.data_ptr(), base, need,
-                                                  torch.cuda.current_stream(dev).cuda_stream)
+                ops.call("b200_vae_decode_temporal", dev, C.byref(d), zf.data_ptr(), n, h, w, int(num_frames), out.data_ptr(), base,
+                         need)
             else:
-                rc = lib.b200_vae_decode(C.byref(d), zf.data_ptr(), n, h, w, out.data_ptr(), base, need,
-                                         torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(rc, "b200_vae_decode")
+                ops.call("b200_vae_decode", dev, C.byref(d), zf.data_ptr(), n, h, w, out.data_ptr(), base, need)
         pd = self.dtype
         out = out if pd == torch.float32 else out.to(pd)
         return DecoderOutput(sample=out) if return_dict else (out,)
