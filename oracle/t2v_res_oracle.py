@@ -72,7 +72,7 @@ def t2v_forward(sd, cfg: T.T2VConfig, x, t, text, dtype=torch.float32, enable_te
     xf = x.permute(0, 2, 1, 3, 4).reshape(B * Fr, C, Hh, Ww).to(dtype)
     patches = xf.reshape(B * Fr, C, gh, p, gw, p).permute(0, 2, 4, 1, 3, 5).reshape(B * Fr, N, C * p * p)
     h = patches @ sd["pos_embed.proj.weight"].to(dtype).reshape(D, -1).t() + sd["pos_embed.proj.bias"].to(dtype)
-    h = h + pos_embed_table(cfg, gh, gw).to(dtype)
+    h = h + pos_embed_table(cfg, gh, gw).to(device=h.device, dtype=dtype)
     ts, emb = T.adaln_single(sd, t, dtype)
     txt = T._lin(sd, "caption_projection.linear_2", F.gelu(T._lin(sd, "caption_projection.linear_1", text.to(dtype)), approximate="tanh"))
     txt_sp = txt.repeat_interleave(Fr, dim=0)
@@ -86,7 +86,7 @@ def t2v_forward(sd, cfg: T.T2VConfig, x, t, text, dtype=torch.float32, enable_te
         if enable_temporal:
             h = h.reshape(B, Fr, N, D).permute(0, 2, 1, 3).reshape(B * N, Fr, D)
             if i == 0 and Fr > 1:
-                h = h + T.temp_pos_embed_table(cfg).to(dtype)
+                h = h + T.temp_pos_embed_table(cfg).to(device=h.device, dtype=dtype)
             h = T.temporal_block(sd, i, h, ts_tm, heads)
             h = h.reshape(B, N, Fr, D).permute(0, 2, 1, 3).reshape(B * Fr, N, D)
     shift, scale = (sd["scale_shift_table"].to(dtype)[None] + emb.repeat_interleave(Fr, dim=0)[:, None]).chunk(2, dim=1)
