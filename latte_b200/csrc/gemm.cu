@@ -558,25 +558,29 @@ int launch_bn(int bf16, int epi, int mn, const GemmMaps& tm, const GemmDev& p, i
 }
 
 constexpr int kStreamKMinKb = 32;          // K / 64 below which the split costs more than the idle tail it removes
+// K / 64 from which a last wave more than half full runs data-parallel: there the second epilogue and reduce-add of every
+// cut tile cost more than the idle tail (DESIGN §6: fc2 of XL/2 at BN 192 on 132 SMs, 2.91 waves of 72 k-blocks)
+constexpr int kStreamKFullTailKb = 64;
 constexpr int kSkFlags = B200_GEMM_SK_FLAGS;   // flags (u64) in the caller's buffer: 4 per streamed tile
 
 int pick_block_n(int M, int N, int K, bool resid, int sms) {
-  // minimise waves x per-tile time.  A tile's cost is modelled by the operand bytes a CTA receives per k-block, A plus
-  // its multicast half of W: 128 + BN/2.
-  // Where the last wave is streamed along K (residual epilogue, long K) there is no wave rounding.
-  // Re-measured with the TMA epilogue on 132 SMs (DESIGN §6): this picks the fastest width for proj and fc1, and widths
-  // 4-6 % slower than 192 for QKV and fc2.  No per-tile cost independent of the SM count picks 192 for QKV on 132 SMs
-  // but keeps 256 on 148 (QKV at 256 / 192: 7 / 9 waves on 132 SMs, 7 / 8 on 148), and the 148-SM choices are kept as
-  // tests/test_schedule.py states them, so the rule is unchanged.
+  // minimise waves x per-tile time, a tile's time being fixed + BN/2.  On 148 SMs it is modelled by the operand bytes a
+  // CTA receives per k-block, A plus its multicast half of W: fixed = 128.  On fewer SMs (H100 SXM: 132) the time of a
+  // wave measured at every width grows nearly in proportion to BN (DESIGN §6: QKV, fc1 and proj with the 16-bit epilogue,
+  // 128 / 192 / 256), so there fixed = 4: it picks 192 for XL/2's QKV, proj and fc2 and 256 for fc1, the fastest widths
+  // measured.  No fixed cost serves both SM counts: QKV runs 7 / 9 waves at 256 / 192 on 132 SMs and 7 / 8 on 148.
+  // Where the last wave is streamed along K (residual epilogue, long K) there is no wave rounding; where plan_gemm keeps
+  // a more than half full last wave data-parallel instead, the rounding it leaves is small and not modelled.
   if (N <= 128) return 128;   // narrow outputs (e.g. the VAE's 3-channel conv_out padded to 32): smallest tile that covers N
   const bool sk = resid && K / BK >= kStreamKMinKb;
+  const int fixed = sms >= 148 ? 128 : 4;
   const int cand[3] = {256, 192, 128};
   int best = 128;
   double best_cost = 1e300;
   for (int i = 0; i < 3; ++i) {
     const long long tiles = static_cast<long long>((M + BM - 1) / BM) * ((N + cand[i] - 1) / cand[i]);
     const double waves = (sk && tiles > sms) ? static_cast<double>(tiles) / sms : static_cast<double>((tiles + sms - 1) / sms);
-    const double cost = waves * (128 + cand[i] / 2);
+    const double cost = waves * (fixed + cand[i] / 2);
     if (cost < best_cost - 1e-9) { best_cost = cost; best = cand[i]; }
   }
   return best;
@@ -600,7 +604,9 @@ GemmPlan plan_gemm(int M, int N, int K, bool resid, int block_n, int sms, int mn
   const int grid = 2 * g.pair_tiles < sms ? 2 * g.pair_tiles : (sms & ~1);   // whole clusters of 2
   g.pairs = grid / 2;
   g.num_kb = K / BK;
-  g.streamk = (resid && g.pair_tiles > g.pairs && g.pair_tiles % g.pairs != 0 && g.num_kb >= kStreamKMinKb) ? 1 : 0;
+  const int tail = g.pair_tiles % g.pairs;     // pair-tiles of the last, partial wave
+  g.streamk = (resid && g.pair_tiles > g.pairs && tail != 0 && g.num_kb >= kStreamKMinKb &&
+               (2 * tail <= g.pairs || g.num_kb < kStreamKFullTailKb)) ? 1 : 0;
   // weight gradients: a small output (fewer tiles than CTA pairs) under a very long contraction (K = tokens).  All tiles are
   // streamed: the (tile, k-block) units are cut into one equal share per pair, a tile's partial sums are reduce-added in k
   // order through the same flags (a chain of waits only ever points from pair p+1 to pair p, and every pair is resident).
