@@ -20,30 +20,19 @@ and the card's name and power limit, read in the same run.
 Usage:  python tools/fp8_step.py [--model latte|t2v] [--frames 16|1] [--steps 30] [--warmup 10] [--rounds 5] [--out DIR]
 """
 import argparse
-import ctypes as C
-import json
 import os
 import re
 import statistics
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
+from harness import card, emit, ms_per_step, profile, require_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim, clk = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim), "max_sm_clock_mhz": float(clk)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
 
 
 def main():
@@ -55,52 +44,27 @@ def main():
     ap.add_argument("--frames", type=int, choices=(16, 1), default=16, help="t2v: video length (1 = text-to-image)")
     ap.add_argument("--out", default=None, help="directory for fp8_step.json (nothing is written without it)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("fp8_step.py measures on a CUDA device; none is visible")
-
-    from latte_b200 import _lib
+    require_cuda()
 
     dev = torch.device("cuda:0")
     setup = setup_t2v if args.model == "t2v" else setup_latte
     workload, nets, step, maxabs = setup(dev, args)
-    res = {"model": args.model, "workload": workload, **card(), "steps": args.steps, "rounds": args.rounds}
+    res = {"model": args.model, "workload": workload, **card(clock=True), "steps": args.steps, "rounds": args.rounds}
     with torch.no_grad():
         for mode, net in nets.items():
             res.setdefault(mode, {})["maxabs_vs_fp32"] = maxabs(net)
             for _ in range(args.warmup):
                 step(net)
-        torch.cuda.synchronize()
         per = {mode: [] for mode in nets}
         for _ in range(args.rounds):
             for mode, net in nets.items():
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(args.steps):
-                    step(net)
-                e1.record()
-                torch.cuda.synchronize()
-                per[mode].append(e0.elapsed_time(e1) / args.steps)
-        lib = _lib.load()
+                per[mode] += ms_per_step(lambda: step(net), args.steps)
         for mode, net in nets.items():
             res[mode]["device_ms_per_step"] = statistics.median(per[mode])
             res[mode]["round_ms"] = [round(v, 4) for v in per[mode]]
-            _lib.profile_enable(True)
-            for _ in range(args.steps):
-                step(net)
-            torch.cuda.synchronize()
-            pm, pn = (C.c_double * 4)(), (C.c_int * 4)()
-            _lib.check(lib.b200_profile_collect(pm, pn, 4), "b200_profile_collect")
-            _lib.profile_enable(False)
-            res[mode]["per_class_ms"] = {k: pm[i] / args.steps for i, k in enumerate(("gemm", "attention", "ln_modulate", "other"))}
-            res[mode]["launches_per_step"] = sum(pn) // args.steps
+            res[mode]["per_class_ms"], res[mode]["launches_per_step"] = profile(lambda: step(net), args.steps)
     res["fp8_speedup"] = res["fp16"]["device_ms_per_step"] / res["fp8"]["device_ms_per_step"]
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        name = "fp8_step.json" if args.model == "latte" else f"fp8_step_t2v_f{args.frames}.json"
-        with open(os.path.join(args.out, name), "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out, "fp8_step.json" if args.model == "latte" else f"fp8_step_t2v_f{args.frames}.json")
 
 
 def setup_latte(dev, args):

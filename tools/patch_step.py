@@ -13,45 +13,26 @@ sample_launches, train_ms (the same over training steps), and the card's name an
 Usage:  python tools/patch_step.py [--patches 2 4 8] [--steps 20] [--warmup 5] [--rounds 5] [--train-batch 4] [--out DIR]
 """
 import argparse
-import ctypes as C
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+
+from harness import card, emit, ms_per_step, profile, require_cuda
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim, clk = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim), "max_sm_clock_mhz": float(clk)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
-
-
 def timed(fn, steps, rounds):
-    """Median over rounds of the mean device time of `steps` back-to-back calls (CUDA events)."""
-    per = []
-    for _ in range(rounds):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize()
-        per.append(e0.elapsed_time(e1) / steps)
+    """Median over rounds of the per-round mean device time, and the rounds."""
+    per = ms_per_step(fn, steps, rounds)
     return statistics.median(per), [round(v, 4) for v in per]
 
 
 def measure(p, args, dev):
-    from latte_b200 import Latte_models, _lib
+    from latte_b200 import Latte_models
     from latte_b200.diffusion import create_diffusion
 
     torch.manual_seed(p)
@@ -72,18 +53,8 @@ def measure(p, args, dev):
         step = lambda: m.forward_with_cfg(x, t, y=y, cfg_scale=4.0)   # noqa: E731
         for _ in range(args.warmup):
             step()
-        torch.cuda.synchronize()
         res["sample_ms"], res["sample_round_ms"] = timed(step, args.steps, args.rounds)
-        lib = _lib.load()
-        _lib.profile_enable(True)
-        for _ in range(args.steps):
-            step()
-        torch.cuda.synchronize()
-        pm, pn = (C.c_double * 4)(), (C.c_int * 4)()
-        _lib.check(lib.b200_profile_collect(pm, pn, 4), "b200_profile_collect")
-        _lib.profile_enable(False)
-    res["sample_per_class_ms"] = {k: pm[i] / args.steps for i, k in enumerate(("gemm", "attention", "ln_modulate", "other"))}
-    res["sample_launches"] = sum(pn) // args.steps
+        res["sample_per_class_ms"], res["sample_launches"] = profile(step, args.steps)
 
     # ---- training: fwd + bwd under bf16 autocast
     m.train()
@@ -100,7 +71,6 @@ def measure(p, args, dev):
         loss.backward()
     for _ in range(max(2, args.warmup // 2)):
         train_step()
-    torch.cuda.synchronize()
     res["train_batch"] = B
     res["train_ms"], res["train_round_ms"] = timed(train_step, max(2, args.steps // 4), args.rounds)
     del m
@@ -117,17 +87,11 @@ def main():
     ap.add_argument("--train-batch", type=int, default=4)
     ap.add_argument("--out", default=None, help="directory for patch_step.json (nothing is written without it)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("patch_step.py measures on a CUDA device; none is visible")
+    require_cuda()
     dev = torch.device("cuda:0")
-    res = {**card(), "workload": "Latte-XL, 16 x 256^2, sampling: CFG pair fp16 graph replay; training: bf16 autocast",
+    res = {**card(clock=True), "workload": "Latte-XL, 16 x 256^2, sampling: CFG pair fp16 graph replay; training: bf16 autocast",
            "models": [measure(p, args, dev) for p in args.patches]}
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "patch_step.json"), "w") as f:
-            f.write(line + "\n")
+    emit(res, args.out, "patch_step.json")
 
 
 if __name__ == "__main__":

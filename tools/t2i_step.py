@@ -11,28 +11,17 @@ Prints one JSON line:
 Usage:  python tools/t2i_step.py [--steps 50] [--warmup 10]
 """
 import argparse
-import ctypes as C
-import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
 import torch
 
+from harness import card, emit, ms_per_step, profile, require_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim, clk = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim), "max_sm_clock_mhz": float(clk)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
 
 
 def main():
@@ -40,8 +29,8 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "t2i_step.py measures on a CUDA device"
-    from latte_b200 import LatteT2V, _lib
+    require_cuda()
+    from latte_b200 import LatteT2V
     from oracle import t2v_oracle as T
 
     dev = torch.device("cuda", 0)
@@ -62,14 +51,7 @@ def main():
     with torch.no_grad():
         for _ in range(W):
             step()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(K):
-            step()
-        e1.record()
-        torch.cuda.synchronize()
-        device_ms = e0.elapsed_time(e1) / K
+        [device_ms] = ms_per_step(step, K)
 
         host = []
         for _ in range(K):
@@ -78,23 +60,14 @@ def main():
             step()
             host.append((time.perf_counter() - t0) * 1e3)
         torch.cuda.synchronize()
-
-        lib = _lib.load()
-        _lib.profile_enable(True)
-        for _ in range(K):
-            step()
-        torch.cuda.synchronize()
-        pm, pn = (C.c_double * 4)(), (C.c_int * 4)()
-        _lib.check(lib.b200_profile_collect(pm, pn, 4), "b200_profile_collect")
-        _lib.profile_enable(False)
+        per_class, launches = profile(step, K, classes=("gemm", "attention", "layernorm", "other"))
 
     res = {"workload": "LatteT2V (Latte-1 config) text-to-image step: 1 x 512 x 512, CFG pair (batch 2), 120 prompt tokens, fp16",
            "steps": K, "warmup": W, "device_ms_per_step": device_ms,
            "host_enqueue_ms": statistics.median(host), "host_enqueue_ms_min": min(host),
-           "per_class_ms": {k: pm[i] / K for i, k in enumerate(("gemm", "attention", "layernorm", "other"))},
-           "launches_per_step": int(sum(pn) // K)}
-    res.update(card())
-    print(json.dumps(res), flush=True)
+           "per_class_ms": per_class, "launches_per_step": launches}
+    res.update(card(clock=True))
+    emit(res)
 
 
 if __name__ == "__main__":

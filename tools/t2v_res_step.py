@@ -17,29 +17,18 @@ and the card's name and power limit, read in the same run.
 Usage:  python tools/t2v_res_step.py [--steps 5] [--warmup 2] [--rounds 3] [--out DIR]
 """
 import argparse
-import ctypes as C
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
+
+from harness import card, emit, ms_per_step, profile, require_cuda
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 SHAPES = [("16x512x512", 16, 64, 64), ("16x320x512", 16, 40, 64), ("16x288x512", 16, 36, 64), ("1x320x512", 1, 40, 64)]
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim, clk = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim), "max_sm_clock_mhz": float(clk)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
 
 
 def main():
@@ -49,10 +38,9 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None, help="directory for t2v_res_step.json (nothing is written without it)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("t2v_res_step.py measures on a CUDA device; none is visible")
+    require_cuda()
 
-    from latte_b200 import LatteT2V, _lib
+    from latte_b200 import LatteT2V
     from oracle import t2v_oracle as T
     from oracle.make_golden_t2v import FULL
 
@@ -78,41 +66,21 @@ def main():
                                                          return_dict=False)[0], 2 * frames * (h // 2) * (w // 2))
 
     res = {"workload": "Latte-1 (LatteT2V, 28 layer pairs, D = 1152) sampling step, batch 2 (CFG pair), 120-token prompt "
-                       "(40 valid), fp16, eager launches", **card(), "steps": args.steps, "rounds": args.rounds}
+                       "(40 valid), fp16, eager launches", **card(clock=True), "steps": args.steps, "rounds": args.rounds}
     with torch.no_grad():
         for step, _ in calls.values():
             for _ in range(args.warmup):
                 step()
-        torch.cuda.synchronize()
         per = {name: [] for name in calls}
         for _ in range(args.rounds):
             for name, (step, _) in calls.items():
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(args.steps):
-                    step()
-                e1.record()
-                torch.cuda.synchronize()
-                per[name].append(e0.elapsed_time(e1) / args.steps)
-        lib = _lib.load()
+                per[name] += ms_per_step(step, args.steps)
         for name, (step, tokens) in calls.items():
             ms = statistics.median(per[name])
             r = res[name] = {"tokens_per_step": tokens, "device_ms_per_step": ms, "ms_per_1k_tokens": ms / (tokens / 1000),
                              "round_ms": [round(v, 3) for v in per[name]]}
-            _lib.profile_enable(True)
-            for _ in range(args.steps):
-                step()
-            torch.cuda.synchronize()
-            pm, pn = (C.c_double * 4)(), (C.c_int * 4)()
-            _lib.check(lib.b200_profile_collect(pm, pn, 4), "b200_profile_collect")
-            _lib.profile_enable(False)
-            r["per_class_ms"] = {k: pm[i] / args.steps for i, k in enumerate(("gemm", "attention", "ln_modulate", "other"))}
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "t2v_res_step.json"), "w") as f:
-            f.write(line + "\n")
+            r["per_class_ms"], _ = profile(step, args.steps)
+    emit(res, args.out, "t2v_res_step.json")
 
 
 if __name__ == "__main__":

@@ -19,17 +19,15 @@ Prints one JSON line per (workload, mode, round):
 Usage:  python tools/train_checkpointing_step.py [--steps 3] [--warmup 1] [--rounds 2]
 """
 import argparse
-import json
 import os
 import sys
 
 import torch
 
+from harness import card, emit, ms_per_step, require_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from train_img_step import card  # noqa: E402
 
 # (model, frames, latent size, batch, modes)
 WORKLOADS = [("latte1", 16, 64, 1, ("plain", "ckpt")), ("latte1", 16, 64, 4, ("ckpt",)), ("latte1", 64, 64, 1, ("ckpt",)),
@@ -93,15 +91,9 @@ def predicted_bytes(m, blocks, width, frames, size, batch, ckpt):
 def measure(step, steps, warmup, dev):
     for _ in range(warmup):
         step()
-    torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats(dev)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps, torch.cuda.max_memory_allocated(dev) / 2 ** 30
+    [ms] = ms_per_step(step, steps)
+    return ms, torch.cuda.max_memory_allocated(dev) / 2 ** 30
 
 
 def main():
@@ -110,7 +102,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--rounds", type=int, default=2, help="alternations of plain / checkpointed where both are measured")
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "train_checkpointing_step.py measures on a CUDA device"
+    require_cuda()
     dev = torch.device("cuda", 0)
     info = card()
     total = torch.cuda.get_device_properties(dev).total_memory
@@ -136,7 +128,7 @@ def main():
                     ms, peak = measure(step, args.steps, max(args.warmup, 1), dev)
                     res.update(steps=args.steps, warmup=args.warmup, ms_per_step=ms, peak_mem_gib=peak)
                 res.update(info)
-                print(json.dumps(res), flush=True)
+                emit(res)
         m.gradient_checkpointing = False
 
 

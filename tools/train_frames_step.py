@@ -12,27 +12,18 @@ Prints one JSON line per frame count:
 Usage:  python tools/train_frames_step.py [--frames 16 32 64] [--steps 5] [--warmup 2]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
+from types import SimpleNamespace
 
 import torch
+
+from harness import Timed, card, emit, ms_per_step, require_cuda
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 BATCH = {16: 4, 32: 2, 64: 1}
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
 
 
 def measure(frames, batch, steps, warmup, dev):
@@ -59,34 +50,19 @@ def measure(frames, batch, steps, warmup, dev):
 
     for _ in range(warmup):
         step()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    [ms] = ms_per_step(step, steps)
 
     ops = m._train_backend[torch.bfloat16]     # the backend object the warm-up steps created
-    events = []
-    plain = ops.attention_bwd
-
-    def timed(qkv, o, do, B, Fr, N, H, temporal):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = plain(qkv, o, do, B, Fr, N, H, temporal)
-        b.record()
-        events.append((temporal, a, b))
-        return r
-
-    ops.attention_bwd = timed
+    # Timed brackets every call of one attribute: route temporal and spatial calls to an attribute each, each timed apart
+    kinds = SimpleNamespace(temporal=ops.attention_bwd, spatial=ops.attention_bwd)
+    timers = [Timed(kinds, "temporal"), Timed(kinds, "spatial")]
+    ops.attention_bwd = lambda qkv, o, do, B, Fr, N, H, temporal: \
+        (kinds.temporal if temporal else kinds.spatial)(qkv, o, do, B, Fr, N, H, temporal)
     for _ in range(steps):
         step()
     torch.cuda.synchronize()
     del ops.attention_bwd
-    tmp = sum(a.elapsed_time(b) for tp, a, b in events if tp) / steps
-    spa = sum(a.elapsed_time(b) for tp, a, b in events if not tp) / steps
+    tmp, spa = (tm.ms() / steps for tm in timers)
     peak = torch.cuda.max_memory_allocated(dev) / 2 ** 30
     del m
     torch.cuda.empty_cache()
@@ -103,14 +79,14 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "train_frames_step.py measures on a CUDA device"
+    require_cuda()
     dev = torch.device("cuda", 0)
     info = card()
     for f in args.frames:
         batch = args.batch or BATCH.get(f, max(1, 64 // f))
         res = measure(f, batch, args.steps, max(args.warmup, 1), dev)
         res.update(info)
-        print(json.dumps(res), flush=True)
+        emit(res)
 
 
 if __name__ == "__main__":

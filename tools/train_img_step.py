@@ -12,53 +12,15 @@ Prints one JSON line per workload:
 Usage:  python tools/train_img_step.py [--steps 5] [--warmup 2]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
 
+from harness import Timed, card, emit, ms_per_step, require_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
-                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, plim = (s.strip() for s in out.strip().splitlines()[0].split(","))
-        return {"gpu": name, "power_limit_w": float(plim)}
-    except Exception as e:  # noqa: BLE001
-        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "nvidia_smi_error": repr(e)[:200]}
-
-
-class _Timed:
-    """Replaces `owner.name` by a wrapper that brackets each call with CUDA events."""
-
-    def __init__(self, owner, name):
-        self.owner, self.name, self.events = owner, name, []
-        self.plain = getattr(owner, name)
-        ev = self.events
-        plain = self.plain
-
-        def timed(*a, **k):
-            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s.record()
-            r = plain(*a, **k)
-            e.record()
-            ev.append((s, e))
-            return r
-        setattr(owner, name, staticmethod(timed) if isinstance(owner, type) else timed)
-
-    def restore(self):
-        if isinstance(self.owner, type):
-            setattr(self.owner, self.name, staticmethod(self.plain))
-        else:
-            delattr(self.owner, self.name)
-
-    def ms(self):
-        return sum(s.elapsed_time(e) for s, e in self.events)
 
 
 def measure(images, batch, frames, steps, warmup, dev):
@@ -89,19 +51,12 @@ def measure(images, batch, frames, steps, warmup, dev):
 
     for _ in range(warmup):
         step()
-    torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats(dev)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    [ms] = ms_per_step(step, steps)
     peak = torch.cuda.max_memory_allocated(dev) / 2 ** 30
 
     ops = m._train_backend[torch.bfloat16]     # the backend object the warm-up steps created
-    timers = [_Timed(ops, "ada_outer"), _Timed(ops, "ada_dsc"), _Timed(training.TrainEngine, "_join_rows")]
+    timers = [Timed(ops, "ada_outer"), Timed(ops, "ada_dsc"), Timed(training.TrainEngine, "_join_rows")]
     for _ in range(steps):
         step()
     torch.cuda.synchronize()
@@ -122,13 +77,13 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "train_img_step.py measures on a CUDA device"
+    require_cuda()
     dev = torch.device("cuda", 0)
     info = card()
     for images, batch in ((8, 4), (0, 5)):
         res = measure(images, batch, 16, args.steps, max(args.warmup, 1), dev)
         res.update(info)
-        print(json.dumps(res), flush=True)
+        emit(res)
 
 
 if __name__ == "__main__":

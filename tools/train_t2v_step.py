@@ -13,17 +13,15 @@ Prints one JSON line per shape:
 Usage:  python tools/train_t2v_step.py [--steps 3] [--warmup 1] [--images 8]
 """
 import argparse
-import json
 import os
 import sys
 
 import torch
 
+from harness import Timed, card, emit, ms_per_step, require_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from train_img_step import _Timed, card  # noqa: E402
 
 SHAPES = [(16, 32, 4), (16, 64, 1), (1, 64, 8)]      # (frames, latent size, batch)
 IMAGE_SHAPES = [(16, 32, 2, False), (16, 64, 1, True)]  # (frames, latent size, batch, gradient checkpointing), with and without images
@@ -51,18 +49,11 @@ def measure(frames, size, batch, steps, warmup, dev, images=0, checkpoint=False)
 
     for _ in range(warmup):
         step()
-    torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats(dev)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        step()
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
+    [ms] = ms_per_step(step, steps)
     peak = torch.cuda.max_memory_allocated(dev) / 2 ** 30
     ops = m._train_backend[torch.bfloat16]
-    timer = _Timed(ops, "cross_attention_bwd")
+    timer = Timed(ops, "cross_attention_bwd")
     for _ in range(steps):
         step()
     torch.cuda.synchronize()
@@ -83,7 +74,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--images", type=int, default=0, help="also time video + image joint training with this many images")
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "train_t2v_step.py measures on a CUDA device"
+    require_cuda()
     dev = torch.device("cuda", 0)
     info = card()
     runs = [(frames, size, batch, 0, False) for frames, size, batch in SHAPES]
@@ -92,7 +83,7 @@ def main():
     for frames, size, batch, images, ckpt in runs:
         res = measure(frames, size, batch, args.steps, max(args.warmup, 1), dev, images, ckpt)
         res.update(info)
-        print(json.dumps(res), flush=True)
+        emit(res)
 
 
 if __name__ == "__main__":
