@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200_ABI_VERSION 8
+#define B200_ABI_VERSION 9
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
 #else
@@ -192,6 +192,36 @@ B200_API size_t b200_t2v_workspace_bytes(const B200T2VShape* shape, int batch, i
 B200_API int b200_t2v_forward(const B200T2VShape* shape, const B200T2VWeights* w, const float* x, const int64_t* t,
                               const float* text, const float* text_bias, int batch, int text_len, int enable_temporal,
                               float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* (ABI v9) Pyramid Attention Broadcast for b200_t2v_forward: an attention module's output is computed on some sampling
+ * steps and reused on others.  One buffer per kind of attention, [layers][T][D] 16-bit in `dtype` (T = batch * frames *
+ * patches per frame, rows in the forward's (b, f, n) order), holds each layer's output of the module's out-projection
+ * (acc + bias), before the gate:
+ *   spatial:  transformer_blocks.l.attn1, added with gate_msa
+ *   temporal: temporal_transformer_blocks.l.attn1, added with its gate_msa
+ *   cross:    transformer_blocks.l.attn2, added with no gate
+ * Modes: COMPUTE runs the module as b200_t2v_forward does and does not touch the buffer; STORE runs it and writes its
+ * pre-gate output into the buffer (whole-K GEMM tiles: the residual stream's fp32 sums may differ from COMPUTE's in
+ * rounding where the out-projection's K would be split); REUSE skips LayerNorm + modulate, QKV, the attention and the
+ * out-projection of every layer and adds gate * buffer into the residual stream.  A cross REUSE also skips the caption
+ * projection and the text K/V GEMM.  A mode outside 0..2, a STORE or REUSE without a buffer, or a buffer that is not
+ * 16-byte aligned is refused (B200_ERR_SHAPE / B200_ERR_ALIGN) before anything is launched.  */
+enum { B200_CACHE_COMPUTE = 0, B200_CACHE_STORE = 1, B200_CACHE_REUSE = 2 };
+typedef struct B200T2VCache {
+  void* spatial;            /* [layers][T][D] 16-bit, or NULL with spatial_mode COMPUTE */
+  void* temporal;
+  void* cross;
+  int32_t spatial_mode;     /* B200_CACHE_* */
+  int32_t temporal_mode;
+  int32_t cross_mode;
+} B200T2VCache;
+
+/* b200_t2v_forward with each kind of attention computed, stored or reused as `cache` says (NULL: every mode COMPUTE,
+ * which is b200_t2v_forward). */
+B200_API int b200_t2v_forward_cached(const B200T2VShape* shape, const B200T2VWeights* w, const float* x, const int64_t* t,
+                                     const float* text, const float* text_bias, int batch, int text_len, int enable_temporal,
+                                     const B200T2VCache* cache, float* out, void* workspace, size_t workspace_bytes,
+                                     void* stream);
 
 /* softmax(q k^T / sqrt(hd) + key_bias) v with K/V from another sequence (diffusers Attention attn2, latte_t2v.py:862-870):
  * q [batch*q_rows_per_batch, q_row_stride] 16-bit (first heads*head_dim columns), kv [batch*kv_len, kv_row_stride]

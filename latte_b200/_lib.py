@@ -10,7 +10,7 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 GEMM_SK_FLAGS = 1024   # B200_GEMM_SK_FLAGS: u64 words of the stream-K flag buffer
 OK = 0
 FP16, BF16 = 0, 1
@@ -52,6 +52,14 @@ T2V_WEIGHT_FIELDS = (
 
 class T2VWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in T2V_WEIGHT_FIELDS]
+
+
+CACHE_COMPUTE, CACHE_STORE, CACHE_REUSE = 0, 1, 2
+
+
+class T2VCache(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("spatial", "temporal", "cross")] + \
+               [(n, C.c_int32) for n in ("spatial_mode", "temporal_mode", "cross_mode")]
 
 
 class T5Shape(C.Structure):
@@ -134,6 +142,9 @@ EXPORTS = {
     "b200_t2v_workspace_bytes": (C.c_size_t, [C.POINTER(T2VShape), C.c_int, C.c_int]),
     "b200_t2v_forward": (C.c_int, [C.POINTER(T2VShape), C.POINTER(T2VWeights), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200_t2v_forward_cached": (C.c_int, [C.POINTER(T2VShape), C.POINTER(T2VWeights), C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(T2VCache), C.c_void_p, C.c_void_p,
+                                          C.c_size_t, C.c_void_p]),
     "b200_cross_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b200_frames_to_uint8": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

@@ -92,12 +92,14 @@ int linear16(const void* A, const void* W, const float* bias, int M, int N, int 
 
 // linear_resid: the gated residual into an fp32 stream, resid[M, N] += gate[(row / rows_per_batch) * gate_bs + col] *
 // (A . W^T + bias), plus row_add[((row / row_add_div) % row_add_period) * N + col] when row_add is set.
+// store16 != NULL: also store16[M, N] = A . W^T + bias in 16 bits (the residual + store epilogue, never stream-K).
 int linear_resid(const void* A, const void* W, const float* bias, int M, int N, int K, int bf16, float* resid,
                  const float* gate, long long gate_bs, int rows_per_batch, unsigned long long* sk_flags, cudaStream_t stream,
-                 const float* row_add = nullptr, int row_add_div = 0, int row_add_period = 0) {
+                 const float* row_add = nullptr, int row_add_div = 0, int row_add_period = 0, void* store16 = nullptr) {
   GemmArgs g{};
-  g.A = A; g.W = W; g.bias = bias; g.M = M; g.N = N; g.K = K; g.bf16 = bf16; g.epilogue = B200_EPI_GATE_RESIDUAL;
-  g.resid = resid; g.gate = gate; g.gate_batch_stride = gate_bs; g.rows_per_batch = rows_per_batch; g.sk_flags = sk_flags;
+  g.A = A; g.W = W; g.bias = bias; g.M = M; g.N = N; g.K = K; g.bf16 = bf16;
+  g.epilogue = store16 ? EPI_GATE_RESIDUAL_STORE16 : B200_EPI_GATE_RESIDUAL; g.out16 = store16;
+  g.resid = resid; g.gate = gate; g.gate_batch_stride = gate_bs; g.rows_per_batch = rows_per_batch; g.sk_flags = store16 ? nullptr : sk_flags;
   g.row_add = row_add; g.row_add_div = row_add_div; g.row_add_period = row_add_period;
   return launch_gemm(g, stream);
 }
@@ -180,9 +182,17 @@ int ln_modulate_linear(const Step& s, const float* shift, const float* scale, co
 }
 
 // m: the block's modulation rows [shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp], each [D]
-int attention_half(const Step& s, const BlockWeights& b, const float* m, int temporal) {
+// cache [T, D] 16-bit, read or written by mode (B200_CACHE_*): STORE also writes the out-projection's acc + bias there;
+// REUSE skips LN + modulate, QKV, the attention and the out-projection and adds gate * cache into x instead.
+int attention_half(const Step& s, const BlockWeights& b, const float* m, int temporal, void* cache = nullptr,
+                   int mode = B200_CACHE_COMPUTE) {
   const int D = s.D;
   cudaStream_t stream = s.stream;
+  if (mode == B200_CACHE_REUSE) {
+    B200_PROF(PROF_OTHER, launch_gate_residual(s.x, cache, m + 2 * D, s.mod_bs, s.F * s.N, nullptr, 0, 0, s.x, s.T(), D, s.bf16,
+                                               stream));
+    return B200_OK;
+  }
   B200_TRY(ln_modulate_linear(s, m + 0 * D, m + 1 * D, b.qkv_w16, b.qkv_w8, b.qkv_ws, b.qkv_b, 3 * D, B200_EPI_BIAS, s.qkv));
   AttnArgs aa{};
   aa.qkv = s.qkv; aa.out = s.h; aa.batch = s.batch; aa.frames = s.F; aa.tokens = s.N; aa.heads = s.heads; aa.head_dim = D / s.heads;
@@ -190,7 +200,7 @@ int attention_half(const Step& s, const BlockWeights& b, const float* m, int tem
   aa.any_len = 1;     // the forwards' shape rules (block_shape_ok) have already decided which spatial lengths they take
   B200_PROF(PROF_ATTN, launch_attention(aa, stream));
   B200_PROF(PROF_GEMM, linear_resid(s.h, b.out_w16, b.out_b, s.T(), D, D, s.bf16, s.x, m + 2 * D, s.mod_bs, s.F * s.N, s.sk_flags,
-                                    stream));
+                                    stream, nullptr, 0, 0, mode == B200_CACHE_STORE ? cache : nullptr));
   return B200_OK;
 }
 
@@ -410,12 +420,31 @@ size_t t2v_carve(const B200T2VShape* s, int batch, int text_len, void* base, T2V
   return a.off;
 }
 
+// every mode is one of B200_CACHE_*, and a mode that stores or reuses has a 16-byte aligned buffer
+int t2v_cache_ok(const B200T2VCache* c) {
+  const void* bufs[3] = {c->spatial, c->temporal, c->cross};
+  const int modes[3] = {c->spatial_mode, c->temporal_mode, c->cross_mode};
+  const char* names[3] = {"spatial", "temporal", "cross"};
+  for (int k = 0; k < 3; ++k) {
+    B200_REQUIRE(modes[k] >= B200_CACHE_COMPUTE && modes[k] <= B200_CACHE_REUSE, B200_ERR_SHAPE, "t2v: %s cache mode %d is not 0, 1 or 2",
+                 names[k], modes[k]);
+    B200_REQUIRE(modes[k] == B200_CACHE_COMPUTE || bufs[k] != nullptr, B200_ERR_SHAPE, "t2v: %s cache mode %d needs a buffer",
+                 names[k], modes[k]);
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(bufs[k]) & 15) == 0, B200_ERR_ALIGN, "t2v: %s cache buffer must be 16-byte aligned",
+                 names[k]);
+  }
+  return B200_OK;
+}
+
 int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, const int64_t* t, const float* text,
-                const float* text_bias, int batch, int text_len, int enable_temporal, float* out, void* workspace,
-                size_t workspace_bytes, cudaStream_t stream) {
+                const float* text_bias, int batch, int text_len, int enable_temporal, const B200T2VCache* cache, float* out,
+                void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   B200_TRY(t2v_shape_ok(s, batch, text_len));
   B200_REQUIRE(w && x && t && text && out && workspace, B200_ERR_SHAPE, "t2v: NULL argument");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 1023) == 0, B200_ERR_ALIGN, "t2v: workspace must be 1024-byte aligned");
+  const B200T2VCache none{};
+  const B200T2VCache& c = cache ? *cache : none;
+  B200_TRY(t2v_cache_ok(&c));
   B200_TRY(check_arch());
   T2VWorkspace ws;
   const size_t need = t2v_carve(s, batch, text_len, workspace, &ws);
@@ -433,6 +462,10 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   const int T = batch * F * N, R = batch * text_len;
   const int bf16 = s->dtype == B200_BF16;
   const long long mod_bs = static_cast<long long>(L) * 2 * 6 * D + 2 * D;
+  // layer l's [T, D] slice of a cache buffer [layers][T][D]
+  const auto cache_layer = [T, D](void* buf, int l) -> void* {
+    return buf ? static_cast<uint16_t*>(buf) + static_cast<size_t>(l) * T * D : nullptr;
+  };
 
   B200_CHECK_CUDA(cudaMemsetAsync(ws.sk_flags, 0, static_cast<size_t>(B200_GEMM_SK_FLAGS) * 8, stream));
   // ---- conditioning (latte_t2v.py:782-784): emb = TimestepEmbedding(sincos(t)); ts = Linear(SiLU(emb)); tables + ts
@@ -441,11 +474,14 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
   B200_PROF(PROF_OTHER, launch_t2v_mod(w->tables, ws.ts, w->final_table, ws.emb, ws.mod, batch, 2 * L, D, stream));
   B200_PROF(PROF_OTHER, launch_fill(ws.ones, 1.0f, D, stream));
 
-  // ---- text: caption projection once per sample (latte_t2v.py:789), then K/V of EVERY layer's cross-attention in one GEMM
-  B200_PROF(PROF_OTHER, launch_cast16(text, ws.text16, static_cast<long long>(R) * s->caption_channels, bf16, stream));
-  B200_PROF(PROF_GEMM, linear16(ws.text16, w->cap_w1_16, w->cap_b1, R, D, s->caption_channels, bf16, B200_EPI_BIAS_GELU, ws.cap_h, stream));
-  B200_PROF(PROF_GEMM, linear16(ws.cap_h, w->cap_w2_16, w->cap_b2, R, D, D, bf16, B200_EPI_BIAS, ws.cap_o, stream));
-  B200_PROF(PROF_GEMM, linear16(ws.cap_o, w->c_kv_w16, w->c_kv_b, R, L * 2 * D, D, bf16, B200_EPI_BIAS, ws.kv_all, stream));
+  // ---- text: caption projection once per sample (latte_t2v.py:789), then K/V of EVERY layer's cross-attention in one GEMM;
+  // only the cross-attention reads them, so a call that reuses its cached outputs skips them
+  if (c.cross_mode != B200_CACHE_REUSE) {
+    B200_PROF(PROF_OTHER, launch_cast16(text, ws.text16, static_cast<long long>(R) * s->caption_channels, bf16, stream));
+    B200_PROF(PROF_GEMM, linear16(ws.text16, w->cap_w1_16, w->cap_b1, R, D, s->caption_channels, bf16, B200_EPI_BIAS_GELU, ws.cap_h, stream));
+    B200_PROF(PROF_GEMM, linear16(ws.cap_h, w->cap_w2_16, w->cap_b2, R, D, D, bf16, B200_EPI_BIAS, ws.cap_o, stream));
+    B200_PROF(PROF_GEMM, linear16(ws.cap_o, w->c_kv_w16, w->c_kv_b, R, L * 2 * D, D, bf16, B200_EPI_BIAS, ws.kv_all, stream));
+  }
 
   // ---- patch embedding + pos_embed (latte_t2v.py:731,773); x arrives as (b c f h w)
   B200_PROF(PROF_OTHER, launch_patch_embed(x, batch, w->patch_w, w->patch_b, w->pos_embed, ws.x, batch, F, s->in_channels,
@@ -457,25 +493,31 @@ int t2v_forward(const B200T2VShape* s, const B200T2VWeights* w, const float* x, 
     // ------------------------------------------------ spatial block (diffusers BasicTransformerBlock; latte_t2v.py:862-870)
     const float* m = ws.mod + static_cast<size_t>(2 * l) * 6 * D;
     const BlockWeights sb = layer(spatial, l, D, HID);
-    B200_TRY(attention_half(st, sb, m, 0));
+    B200_TRY(attention_half(st, sb, m, 0, cache_layer(c.spatial, l), c.spatial_mode));
     // cross-attention on the UN-normalised stream (no norm2 before attn2 in ada_norm_single mode), residual without gate
-    B200_PROF(PROF_OTHER, launch_cast16(ws.x, ws.h, static_cast<long long>(T) * D, bf16, stream));
-    B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->c_q_w16) + l * DD, w->c_q_b + static_cast<size_t>(l) * D, T, D,
-                                  D, bf16, B200_EPI_BIAS, ws.qkv, stream));
-    CrossAttnArgs ca{};
-    ca.q = ws.qkv; ca.kv = ws.kv_all + static_cast<size_t>(l) * 2 * D; ca.out = ws.h; ca.batch = batch; ca.q_rows_per_batch = F * N;
-    ca.kv_len = text_len; ca.q_row_stride = D; ca.kv_row_stride = L * 2 * D; ca.heads = H; ca.head_dim = D / H; ca.bf16 = bf16;
-    ca.key_bias = text_bias;     // padded prompts: (1 - mask) * -10000 per text token (latte_t2v.py:766-771), or NULL
-    B200_PROF(PROF_ATTN, launch_cross_attention(ca, stream));
-    B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->c_out_w16) + l * DD, w->c_out_b + static_cast<size_t>(l) * D,
-                                      T, D, D, bf16, ws.x, ws.ones, 0, F * N, ws.sk_flags, stream));
+    void* cross = cache_layer(c.cross, l);
+    if (c.cross_mode == B200_CACHE_REUSE) {
+      B200_PROF(PROF_OTHER, launch_gate_residual(ws.x, cross, ws.ones, 0, F * N, nullptr, 0, 0, ws.x, T, D, bf16, stream));
+    } else {
+      B200_PROF(PROF_OTHER, launch_cast16(ws.x, ws.h, static_cast<long long>(T) * D, bf16, stream));
+      B200_PROF(PROF_GEMM, linear16(ws.h, static_cast<const uint16_t*>(w->c_q_w16) + l * DD, w->c_q_b + static_cast<size_t>(l) * D, T, D,
+                                    D, bf16, B200_EPI_BIAS, ws.qkv, stream));
+      CrossAttnArgs ca{};
+      ca.q = ws.qkv; ca.kv = ws.kv_all + static_cast<size_t>(l) * 2 * D; ca.out = ws.h; ca.batch = batch; ca.q_rows_per_batch = F * N;
+      ca.kv_len = text_len; ca.q_row_stride = D; ca.kv_row_stride = L * 2 * D; ca.heads = H; ca.head_dim = D / H; ca.bf16 = bf16;
+      ca.key_bias = text_bias;     // padded prompts: (1 - mask) * -10000 per text token (latte_t2v.py:766-771), or NULL
+      B200_PROF(PROF_ATTN, launch_cross_attention(ca, stream));
+      B200_PROF(PROF_GEMM, linear_resid(ws.h, static_cast<const uint16_t*>(w->c_out_w16) + l * DD, w->c_out_b + static_cast<size_t>(l) * D,
+                                        T, D, D, bf16, ws.x, ws.ones, 0, F * N, ws.sk_flags, stream, nullptr, 0, 0,
+                                        c.cross_mode == B200_CACHE_STORE ? cross : nullptr));
+    }
     // + temp_pos_embed before the first temporal block (latte_t2v.py:894-895), folded into this epilogue
     B200_TRY(mlp_half(st, sb, m, (l == 0 && enable_temporal && F > 1) ? w->temp_embed : nullptr));
     if (!enable_temporal) continue;
     // ------------------------------------------------ temporal block (BasicTransformerBlock_, latte_t2v.py:897-905)
     const float* mt = ws.mod + static_cast<size_t>(2 * l + 1) * 6 * D;
     const BlockWeights tb = layer(temporal, l, D, HID);
-    B200_TRY(attention_half(st, tb, mt, 1));
+    B200_TRY(attention_half(st, tb, mt, 1, cache_layer(c.temporal, l), c.temporal_mode));
     B200_TRY(mlp_half(st, tb, mt, nullptr));
   }
 
@@ -677,6 +719,7 @@ B200_API int b200_linear(const void* A, const void* W, const float* bias, int M,
                 void* out16, float* resid, const float* gate, int64_t gate_batch_stride, int rows_per_batch,
                 int block_n, void* sk_flags, void* stream) {
   B200_REQUIRE(dtype == B200_FP16 || dtype == B200_BF16, B200_ERR_DTYPE, "dtype %d unknown", dtype);
+  B200_REQUIRE(epilogue != b200::EPI_GATE_RESIDUAL_STORE16, B200_ERR_UNSUPPORTED, "gemm: unknown epilogue %d", epilogue);
   B200_REQUIRE((reinterpret_cast<uintptr_t>(sk_flags) & 7) == 0, B200_ERR_ALIGN, "sk_flags must be 8-byte aligned");
   b200::GemmArgs a{};
   a.sk_flags = static_cast<unsigned long long*>(sk_flags);
@@ -710,12 +753,21 @@ B200_API size_t b200_t2v_workspace_bytes(const B200T2VShape* shape, int batch, i
   return b200::t2v_carve(shape, batch, text_len, nullptr, &ws);
 }
 
+B200_API int b200_t2v_forward_cached(const B200T2VShape* shape, const B200T2VWeights* w, const float* x, const int64_t* t,
+                                     const float* text, const float* text_bias, int batch, int text_len, int enable_temporal,
+                                     const B200T2VCache* cache, float* out, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  B200_REQUIRE(!text_bias || (reinterpret_cast<uintptr_t>(text_bias) & 15) == 0, B200_ERR_ALIGN, "t2v: text_bias must be 16-byte aligned");
+  return b200::t2v_forward(shape, w, x, t, text, text_bias, batch, text_len, enable_temporal, cache, out, workspace,
+                           workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
 B200_API int b200_t2v_forward(const B200T2VShape* shape, const B200T2VWeights* w, const float* x, const int64_t* t,
                               const float* text, const float* text_bias, int batch, int text_len, int enable_temporal,
                               float* out, void* workspace, size_t workspace_bytes, void* stream) {
-  B200_REQUIRE(!text_bias || (reinterpret_cast<uintptr_t>(text_bias) & 15) == 0, B200_ERR_ALIGN, "t2v: text_bias must be 16-byte aligned");
-  return b200::t2v_forward(shape, w, x, t, text, text_bias, batch, text_len, enable_temporal, out, workspace, workspace_bytes,
-                           static_cast<cudaStream_t>(stream));
+  const B200T2VCache compute{};   // every attention computed, nothing stored
+  return b200_t2v_forward_cached(shape, w, x, t, text, text_bias, batch, text_len, enable_temporal, &compute, out, workspace,
+                                 workspace_bytes, stream);
 }
 
 B200_API int b200_cross_attention(const void* q, const void* kv, const float* key_bias, void* out, int batch, int q_rows_per_batch,

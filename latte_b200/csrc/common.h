@@ -90,7 +90,7 @@ struct GemmArgs {
   int M, N, K;
   int bf16;             // 0 = fp16 operands, 1 = bf16
   int epilogue;         // B200_EPI_*
-  void* out16;          // [M, N] 16-bit   (EPI_BIAS / EPI_BIAS_GELU)
+  void* out16;          // [M, N] 16-bit   (EPI_BIAS / EPI_BIAS_GELU; EPI_GATE_RESIDUAL_STORE16: acc + bias)
   float* resid;         // [M, N] fp32 in/out (EPI_GATE_RESIDUAL): resid += gate * (acc + bias) (+ row_add)
   const float* gate;    // gate[(row / rows_per_batch) * gate_batch_stride + col]
   long long gate_batch_stride;
@@ -110,6 +110,9 @@ struct GemmArgs {
   int conv_taps, conv_n, conv_h, conv_w, conv_c;
   int conv_dx[9], conv_dy[9], conv_dz[9];   // dz shifts the image index (temporal convolution over the frames of one clip)
 };
+// Internal epilogue (not a b200_linear value): B200_EPI_GATE_RESIDUAL plus out16[M, N] = acc + bias in 16 bits, on
+// whole-K tiles (no stream-K).  LatteT2V's attention cache (b200_t2v_forward_cached) stores its entries with it.
+constexpr int EPI_GATE_RESIDUAL_STORE16 = 6;
 int launch_gemm(const GemmArgs& a, cudaStream_t stream);
 // FP8 forward GEMM: out16[M, N] = epi(a_scale[row] * w_scale[col] * (A8[M, K] . W8[N, K]^T) + bias), both operands e4m3
 // K-major, epilogue B200_EPI_BIAS or B200_EPI_BIAS_GELU, K % 16 == 0 (16-byte rows), N % 32 == 0

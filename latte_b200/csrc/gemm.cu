@@ -26,6 +26,9 @@
 //   residual:        32-column fp32 chunks of the increment gate * (acc + bias) (+ row_add); x is never loaded: a
 //                    cp.reduce.async.bulk.tensor .add folds the chunk into the fp32 residual stream in L2, once per GEMM --
 //                    or, for the stream-K tiles of the last waves, once per K segment in k order (TileSched below).
+//   residual + store: the residual epilogue, and beside each fp32 chunk the 16-bit acc + bias of the same 32 columns,
+//                    staged in a buffer of its own and written by a second TMA store (resid_store_gemm: LatteT2V's
+//                    attention cache, DESIGN.md §13).  Whole-K tiles only: a stream-K segment never holds the whole sum.
 #include <cstdio>
 #include "common.h"
 #include "ptx.cuh"
@@ -47,19 +50,23 @@ constexpr int kConsumerRegs = 232;
 
 // epilogue staging buffer: 64 rows x 128 bytes (32 fp32 or 64 16-bit columns), two per consumer warpgroup
 constexpr int kEpiBufBytes = 64 * 128;
+// the residual + store epilogue's second staging buffer: 64 rows x 64 bytes (32 16-bit columns), two per consumer warpgroup
+constexpr int kEpi16BufBytes = 64 * 64;
 
 template <int BN, int EPI>
 struct Cfg {
   static constexpr int BLOCK_N = BN;
-  static constexpr bool RESID = EPI == B200_EPI_GATE_RESIDUAL;
+  static constexpr bool STORE16 = EPI == EPI_GATE_RESIDUAL_STORE16;  // residual, plus acc + bias in 16 bits
+  static constexpr bool RESID = EPI == B200_EPI_GATE_RESIDUAL || STORE16;
   static constexpr bool TWO_OUT = EPI == B200_EPI_BIAS_GELU_BOTH;   // out16 and out16b
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;                       // the whole W tile (both CTAs' halves)
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_BYTES = 2 * 2 * kEpiBufBytes;            // 2 consumer warpgroups x 2 buffers = 32 KiB
+  // 2 consumer warpgroups x 2 buffers = 32 KiB (+ 16 KiB of 16-bit buffers with STORE16)
+  static constexpr int EPI_BYTES = 2 * 2 * kEpiBufBytes + (STORE16 ? 2 * 2 * kEpi16BufBytes : 0);
   static constexpr int BAR_BYTES = 256;
   static constexpr int STAGES_FIT = (232448 - EPI_BYTES - BAR_BYTES - 1024) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // BN 256: 4, 192: 4, 128: 6
+  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // BN 256: 4, 192: 4, 128: 6 (STORE16: 3, 4, 5)
   static constexpr int EPI_OFF = STAGES * STAGE_BYTES;             // 1 KiB aligned: the buffers keep the swizzle phase
   static constexpr int BAR_OFF = EPI_OFF + EPI_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFF + BAR_BYTES + 1024;    // +1024: manual 1 KiB alignment of the base
@@ -354,19 +361,21 @@ struct Consumer {
 // wgrad uses 3 (dW = dY^T X), dgrad 2 (dX = dY W with W in its [out, in] layout), everything else 0.  A compile-time
 // layout keeps one straight-line wgmma sequence per k-block: a run-time choice between four makes ptxas join them with
 // an injected empty wgmma group, which turns wgmma_wait<1> into a full drain.
+// The body of gemm_kernel and resid_store_gemm, inlined into each: one kernel name per epilogue family keeps the
+// instances of gemm_kernel exactly those its callers launched before the residual + store epilogue existed.
 template <int BN, int EPI, bool BF16, int MN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmDev p) {
-  // tmC: the output, fp32 resid [M, N] (box 32 x 64) or 16-bit out16 [M, N] (box 64 x 64); tmC2: out16b (GELU_BOTH only)
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                                          const CUtensorMap& tmC2, const GemmDev& p) {
+  // tmC: the output, fp32 resid [M, N] (box 32 x 64) or 16-bit out16 [M, N] (box 64 x 64); tmC2: out16b (GELU_BOTH) or
+  // the 16-bit acc + bias [M, N] (box 32 x 64, STORE16)
   using C = Cfg<BN, EPI>;
   constexpr int TA = MN & 1, TB = MN >> 1;
   static_assert(MN == 0 || MN == 2 || MN == 3, "operand layouts: 0 forward, 2 dgrad, 3 wgrad");
   const int warp = threadIdx.x >> 5;
-  const Pipeline<C> pl = C::TWO_OUT ? gemm_prologue<C>(&tmA, &tmB, &tmC, &tmC2) : gemm_prologue<C>(&tmA, &tmB, &tmC);
+  const Pipeline<C> pl = (C::TWO_OUT || C::STORE16) ? gemm_prologue<C>(&tmA, &tmB, &tmC, &tmC2) : gemm_prologue<C>(&tmA, &tmB, &tmC);
   const PairTiles<BN> pt(p);
   const int num_kb = p.K / BK;
-  const bool streamk = C::RESID && p.streamk != 0;
+  const bool streamk = C::RESID && !C::STORE16 && p.streamk != 0;
 
   if (warp < 4) {
     produce(pl, pt, num_kb, streamk, [&](uint8_t* sa, uint64_t* bar, int m_blk, int w_row0, int kb) {
@@ -447,6 +456,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (n0 + 32 * c >= p.N) break;       // N % 32 == 0: a chunk lies wholly inside N or wholly past it
           uint8_t* buf = cs.epi + (2 * cs.wg + (cs.ep & 1)) * kEpiBufBytes;
           const uint32_t buf_addr = smem_u32(buf);
+          // STORE16: this chunk's 16-bit acc + bias, 64 rows x 64 bytes unswizzled, after the four fp32 buffers
+          uint8_t* buf16 = cs.epi + 4 * kEpiBufBytes + (2 * cs.wg + (cs.ep & 1)) * kEpi16BufBytes;
+          const uint32_t buf16_addr = smem_u32(buf16);
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
             const int j = 4 * c + jj, col = n0 + 8 * j + 2 * cs.cq;
@@ -459,6 +471,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               const float d1 = resid_delta(acc[4 * j + 2 * h + 1], b2.y, gt.y, ra.y, add_row[h] != nullptr);
               // buffer row lr0 + 8h is 128 bytes; its 16-byte units are XOR-swizzled by the row % 8 (= g), as SW128 TMA reads them
               st_shared_f2(buf_addr + (cs.lr0 + 8 * h) * 128 + (((2 * jj + (cs.cq >> 1)) ^ cs.g) << 4) + 8 * (cs.cq & 1), d0, d1);
+              if constexpr (C::STORE16) {
+                const uint32_t v = pack2<BF16>(__fadd_rn(acc[4 * j + 2 * h], b2.x), __fadd_rn(acc[4 * j + 2 * h + 1], b2.y));
+                st_shared_u32(buf16_addr + (cs.lr0 + 8 * h) * 64 + 16 * jj + 4 * cs.cq, v);
+              }
             }
           }
           fence_proxy_async_smem();            // the writes above -> visible to TMA
@@ -472,6 +488,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               ordered = true;
             }
             tma_reduce_add_2d(&tmC, buf, n0 + 32 * c, m0w);
+            if constexpr (C::STORE16) tma_store_2d(&tmC2, buf16, n0 + 32 * c, m0w);
             tma_store_commit();
             tma_store_wait_read<1>();          // the previous chunk has been read out of the other buffer ...
           }
@@ -517,13 +534,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   cluster_sync_all();   // the peer may still multicast into our smem / arrive on our barriers until it is done too
 }
 
-// the kernel's four tensor maps: operands A and W, output (resid or out16) and second output (out16b)
+template <int BN, int EPI, bool BF16, int MN>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmDev p) {
+  static_assert(EPI != EPI_GATE_RESIDUAL_STORE16, "the residual + store epilogue is resid_store_gemm");
+  gemm_body<BN, EPI, BF16, MN>(tmA, tmB, tmC, tmC2, p);
+}
+
+// the residual + store epilogue, K-major operands: resid += gate * (acc + bias) and out16 = acc + bias (16 bits)
+template <int BN, bool BF16>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+resid_store_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmDev p) {
+  gemm_body<BN, EPI_GATE_RESIDUAL_STORE16, BF16, 0>(tmA, tmB, tmC, tmC2, p);
+}
+
+// the kernel's four tensor maps: operands A and W, output (resid or out16) and second output (out16b, or STORE16's out16)
 struct GemmMaps { CUtensorMap a, b, c, c2; };
 
 template <int BN, int EPI, bool BF16, int MN>
 int launch_one(const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t stream) {
   using C = Cfg<BN, EPI>;
   auto kern = gemm_kernel<BN, EPI, BF16, MN>;
+  B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
+  B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tm.a, tm.b, tm.c, tm.c2, p));
+  return B200_OK;
+}
+
+template <int BN, bool BF16>
+int launch_resid_store(const GemmMaps& tm, const GemmDev& p, int grid, cudaStream_t stream) {
+  using C = Cfg<BN, EPI_GATE_RESIDUAL_STORE16>;
+  auto kern = resid_store_gemm<BN, BF16>;
   B200_SET_SMEM_ONCE(kern, C::SMEM_BYTES);
   B200_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(kThreads), C::SMEM_BYTES, stream, tm.a, tm.b, tm.c, tm.c2, p));
   return B200_OK;
@@ -542,6 +584,7 @@ int launch_epi(int epi, int mn, const GemmMaps& tm, const GemmDev& p, int grid, 
       case B200_EPI_BIAS_ADD16: return launch_one<BN, B200_EPI_BIAS_ADD16, BF16, 0>(tm, p, grid, s);
       case B200_EPI_BIAS_MUL16: return launch_one<BN, B200_EPI_BIAS_MUL16, BF16, 0>(tm, p, grid, s);
       case B200_EPI_BIAS_GELU_BOTH: return launch_one<BN, B200_EPI_BIAS_GELU_BOTH, BF16, 0>(tm, p, grid, s);
+      case EPI_GATE_RESIDUAL_STORE16: return launch_resid_store<BN, BF16>(tm, p, grid, s);
     }
   }
   if constexpr (BN != 192) {
@@ -774,8 +817,11 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   B200_REQUIRE(a.K % BK == 0, B200_ERR_SHAPE, "gemm: K=%d must be a multiple of %d", a.K, BK);
   B200_REQUIRE(a.N % 32 == 0, B200_ERR_SHAPE, "gemm: N=%d must be a multiple of 32", a.N);
   B200_REQUIRE(a.epilogue == B200_EPI_BIAS || a.epilogue == B200_EPI_BIAS_GELU || a.epilogue == B200_EPI_GATE_RESIDUAL ||
-                   a.epilogue == B200_EPI_BIAS_ADD16 || a.epilogue == B200_EPI_BIAS_MUL16 || a.epilogue == B200_EPI_BIAS_GELU_BOTH,
+                   a.epilogue == B200_EPI_BIAS_ADD16 || a.epilogue == B200_EPI_BIAS_MUL16 || a.epilogue == B200_EPI_BIAS_GELU_BOTH ||
+                   a.epilogue == EPI_GATE_RESIDUAL_STORE16,
                B200_ERR_UNSUPPORTED, "gemm: unknown epilogue %d", a.epilogue);
+  B200_REQUIRE(a.epilogue != EPI_GATE_RESIDUAL_STORE16 || (a.mn_major == 0 && a.conv_taps == 0), B200_ERR_UNSUPPORTED,
+               "gemm: the residual + store epilogue takes K-major operands only");
   B200_REQUIRE((a.epilogue != B200_EPI_BIAS_ADD16 && a.epilogue != B200_EPI_BIAS_MUL16) ||
                    (a.add16 && (reinterpret_cast<uintptr_t>(a.add16) & 15) == 0), B200_ERR_ALIGN, "gemm: add16 tensor missing or unaligned");
   B200_REQUIRE(a.epilogue != B200_EPI_BIAS_GELU_BOTH || (a.out16b && (reinterpret_cast<uintptr_t>(a.out16b) & 15) == 0), B200_ERR_ALIGN,
@@ -783,7 +829,10 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   B200_REQUIRE(a.epilogue != B200_EPI_BIAS_GELU_BOTH || a.N % 8 == 0, B200_ERR_SHAPE, "gemm: N %% 8");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(a.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.W) & 15) == 0,
                B200_ERR_ALIGN, "gemm: A and W must be 16-byte aligned");
-  const bool resid = a.epilogue == B200_EPI_GATE_RESIDUAL;
+  const bool store16 = a.epilogue == EPI_GATE_RESIDUAL_STORE16;
+  const bool resid = a.epilogue == B200_EPI_GATE_RESIDUAL || store16;
+  B200_REQUIRE(!store16 || (a.out16 && (reinterpret_cast<uintptr_t>(a.out16) & 15) == 0), B200_ERR_ALIGN,
+               "gemm: the residual + store epilogue needs a 16-byte aligned out16");
   if (resid) {
     B200_REQUIRE(a.resid && a.gate && a.rows_per_batch > 0, B200_ERR_SHAPE, "gemm: gated-residual epilogue needs resid, gate, rows_per_batch");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(a.resid) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.gate) & 15) == 0 &&
@@ -857,6 +906,10 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
       const uint32_t boxC[2] = {32, 64};
       B200_TRY(make_tmap(&tm.c, a.resid, 4, 2, dimsC, strC, boxC, TMAP_SW_128));
       tm.c2 = tm.c;
+      if (store16) {   // 32 16-bit columns x 64 rows per chunk, the same box as the fp32 chunk, unswizzled
+        const uint64_t str16[1] = {static_cast<uint64_t>(a.N) * 2};
+        B200_TRY(make_tmap_16bit(&tm.c2, a.out16, 2, dimsC, str16, boxC, TMAP_SW_NONE));
+      }
     } else {
       B200_TRY(make_out16_map(&tm.c, a.out16, a.M, a.N));
       if (a.epilogue == B200_EPI_BIAS_GELU_BOTH) B200_TRY(make_out16_map(&tm.c2, a.out16b, a.M, a.N));
@@ -888,7 +941,8 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
     // the ordering flags live in the CALLER's buffer (zeroed once; every launch leaves it zeroed): without one the
     // schedule stays data-parallel
     const int streamed = pair_tiles % pairs + pairs;  // tiles of the partial wave and of the full wave before it
-    p.streamk = (plan.streamk && a.sk_flags != nullptr && streamed * 4 <= kSkFlags) ? 1 : 0;
+    // (the residual + store epilogue needs each tile's whole sum: it never streams)
+    p.streamk = (plan.streamk && !store16 && a.sk_flags != nullptr && streamed * 4 <= kSkFlags) ? 1 : 0;
     p.sk_flags = p.streamk ? a.sk_flags : nullptr;
   }
   switch (bn) {

@@ -202,6 +202,10 @@ __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const vo
 __device__ __forceinline__ void st_shared_f2(uint32_t saddr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
 }
+// 4-byte shared-memory store through a shared-window address
+__device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
 // four 8x8 16-bit matrices to shared memory: register i of lane (4g + q) holds row g, columns 2q, 2q + 1 of matrix i (the
 // wgmma / mma accumulator fragment once packed); lane l gives the address of row l % 8 of matrix l / 8 (16 bytes)
 __device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
